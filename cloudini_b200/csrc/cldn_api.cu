@@ -260,6 +260,7 @@ const char* dev_error_text(uint32_t code) {
     case DEV_ERR_OUTPUT_SMALL: return "Output buffer is too small to hold the decoded data";
     case DEV_ERR_ENCODE_OUTPUT_SMALL: return "Output buffer too small for uncompressed chunk";  // chunk_writer.cpp:33-35
     case DEV_ERR_LZ4: return "LZ4 decompression failed";  // codec_common.cpp:279-281
+    case DEV_ERR_ZSTD: return "ZSTD decompression failed";  // codec_common.cpp:290-293
     default: return "unknown device error";
   }
 }
@@ -867,6 +868,7 @@ struct cldn_decoder {
   PinBuf<uint64_t> h_lz_sizes;
   PinRing<Lz4Frame> h_lz_frames;
   PinRing<uint32_t> h_lz_chunk_frame;
+  DevBuf<uint8_t> d_zs_lit;        // ZSTD: literal scratch per decompressing warp
   bool fast_launched = false;  // the last batch went through decode_floatn_fast_kernel (cldn_b200_decoder_last_stats)
   uint32_t fast_chunks = 0;
   bool sections_ahead = false;    // the last batch ran in side mode (cldn_b200_decoder_last_sections_ahead)
@@ -895,7 +897,7 @@ static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
     return CLDN_ERR_UNSUPPORTED;
   }
   if (info.compression_opt != CLDN_COMP_NONE) {
-    set_error("compression_opt %d: stage 2 is undone before the stage-1 decode (LZ4 on the device, ZSTD by the host library)", static_cast<int>(info.compression_opt));
+    set_error("compression_opt %d: stage 2 is undone before the stage-1 decode (LZ4 and ZSTD on the device)", static_cast<int>(info.compression_opt));
     return CLDN_ERR_UNSUPPORTED;
   }
   if (info.version < 3) { set_error("wire version %d (single unframed chunk) is not supported", info.version); return CLDN_ERR_UNSUPPORTED; }
@@ -1105,7 +1107,7 @@ void cldn_b200_decoder_destroy(cldn_decoder_t* d) {
   d->d_err.release(); d->h_err.release(); d->d_in.release(); d->d_out.release();
   d->d_chunk_tiles.release(); d->d_chunk_tile_begin.release(); d->d_stream_end.release(); d->d_tsums.release(); d->d_tstatus.release(); d->d_chunk_frame.release(); d->d_tile_chunk.release(); d->d_trace.release(); d->d_counter.release(); d->d_redo.release(); d->d_side.release(); d->d_chunk_desc.release(); d->pipe.release();
   d->d_s1.release(); d->d_lz_scratch.release(); d->d_lz_chunk_frame.release(); d->d_lz_chunk_sizes.release(); d->d_lz_frames.release();
-  d->d_lz_sizes.release(); d->h_lz_sizes.release(); d->h_lz_frames.release(); d->h_lz_chunk_frame.release();
+  d->d_lz_sizes.release(); d->h_lz_sizes.release(); d->h_lz_frames.release(); d->h_lz_chunk_frame.release(); d->d_zs_lit.release();
   if (d->own_stream && d->stream) cudaStreamDestroy(d->stream);
   delete d;
 }
@@ -1212,6 +1214,154 @@ static int decode_batch_device_lz4(cldn_decoder* d, const cldn_info_t& info, siz
   return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities);
 }
 
+// Bound of one decompressed chunk, as the host-pointer API has always passed it to ZSTD_decompress / LZ4_decompress_safe:
+// the stage-1 worst case of a chunk, or the whole frame's bytes if larger (DecompressChunk's bound is w*h*step,
+// cloudini.cpp:672-675), plus 64.
+static size_t stage2_max_body(const cldn_info_t& info, bool* ok) {
+  cldn_info_t plain = info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  const size_t pts = static_cast<size_t>(info.width) * info.height;
+  const size_t m = max_compressed_size(plain, std::min<size_t>(pts, kChunkPoints), false, ok);
+  return std::max<size_t>(m, pts * info.point_step) + 64;
+}
+
+// CLDN_B200_ZSTD_HOST=1: the host-pointer API decompresses ZSTD with the system libzstd, chunk after chunk, as before the
+// device decompressor existed (a comparison / bisecting aid).
+static bool zstd_host_route() {
+  const char* v = getenv("CLDN_B200_ZSTD_HOST");
+  return v && v[0] == '1';
+}
+
+// Device pointers, compression ZSTD: the LZ4 path's structure (slots, chunk table, re-framing) with the ZSTD decompressor
+// of cldn_zstd.cu. A chunk may decompress to max_body bytes (the host-pointer bound) but not beyond its slot, which holds
+// the stage-1 worst case of a 32768-point chunk: a larger chunk body cannot be a stage-1 chunk and is refused as damaged.
+// On return p1 / b1 are the frames' stage-1 payloads in the internal arena (one read-back of their sizes).
+static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads, const size_t* payload_bytes,
+                              std::vector<const void*>& p1, std::vector<size_t>& b1) {
+  cldn_info_t plain = info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
+  if (n_points > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
+  bool ok;
+  const size_t max_body = stage2_max_body(info, &ok);
+  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
+  const size_t chunks_per_frame = static_cast<size_t>((n_points + kChunkPoints - 1) / kChunkPoints);
+  const size_t chunk_worst = max_compressed_size(plain, std::min<size_t>(n_points, kChunkPoints), false, &ok) + 64;
+  const size_t cap = std::min(max_body, chunk_worst);
+  const size_t slot = (cap + 15) & ~size_t(15);
+  const size_t s1_cap = ((chunks_per_frame * (slot + 4) + 255) & ~size_t(255));
+  const size_t chunks = chunks_per_frame * n_frames;
+  if (chunks > 0x7FFFFFFFull || slot > 0xFFFFFFF0ull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
+  for (size_t f = 0; f < n_frames; ++f) {  // a frame without points has no chunk to decompress
+    if (chunks_per_frame == 0 && payload_bytes[f] != 0) { set_error("%s", dev_error_text(DEV_ERR_CHUNK_COUNT)); return CLDN_ERR_CORRUPT_DATA; }
+  }
+  // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
+  const uint32_t wpc = zstd_warps_per_cta();
+  const size_t ctas = std::max<size_t>(1, std::min<size_t>((chunks + wpc - 1) / wpc, 2048 / wpc));
+  const size_t lit_stride = zstd_lit_scratch_bytes(static_cast<uint32_t>(cap));
+  if (int rc = d->d_s1.reserve(std::max<size_t>(s1_cap * n_frames, 256))) return rc;
+  if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
+  if (int rc = d->d_zs_lit.reserve(ctas * wpc * lit_stride)) return rc;
+  if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
+  if (int rc = d->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
+  if (int rc = d->d_lz_frames.reserve(n_frames)) return rc;
+  if (int rc = d->d_lz_sizes.reserve(n_frames)) return rc;
+  if (int rc = d->h_lz_sizes.reserve(n_frames)) return rc;
+  Lz4Frame* hf = nullptr; int hf_slot = 0;
+  uint32_t* hcf = nullptr; int hcf_slot = 0;
+  if (int rc = d->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
+  if (int rc = d->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
+  for (size_t f = 0; f < n_frames; ++f) {
+    Lz4Frame& F = hf[f];
+    memset(&F, 0, sizeof(F));
+    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
+    F.packed_in_bytes = payload_bytes[f];
+    F.plain_out = d->d_s1.p + f * s1_cap;
+    F.plain_cap = s1_cap;
+    F.n_chunks = static_cast<uint32_t>(chunks_per_frame);
+    F.chunk_begin = static_cast<uint32_t>(f * chunks_per_frame);
+    for (size_t c = 0; c < chunks_per_frame; ++c) hcf[f * chunks_per_frame + c] = static_cast<uint32_t>(f);
+  }
+  CUDA_TRY(cudaMemcpyAsync(d->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, d->stream));
+  if (int rc = d->h_lz_frames.commit(hf_slot, d->stream)) return rc;
+  if (chunks) CUDA_TRY(cudaMemcpyAsync(d->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
+  if (int rc = d->h_lz_chunk_frame.commit(hcf_slot, d->stream)) return rc;
+  ZstdLaunch Z;
+  memset(&Z, 0, sizeof(Z));
+  Z.L.frames = d->d_lz_frames.p;
+  Z.L.n_frames = static_cast<uint32_t>(n_frames);
+  Z.L.n_chunks_total = static_cast<uint32_t>(chunks);
+  Z.L.chunk_frame = d->d_lz_chunk_frame.p;
+  Z.L.scratch = d->d_lz_scratch.p;
+  Z.L.slot_stride = static_cast<uint32_t>(slot);
+  Z.L.chunk_sizes = d->d_lz_chunk_sizes.p;
+  Z.L.sizes = d->d_lz_sizes.p;
+  Z.L.err = d->d_err.p;
+  Z.body_cap = static_cast<uint32_t>(cap);
+  Z.n_ctas = static_cast<uint32_t>(ctas);
+  Z.lit_scratch = d->d_zs_lit.p;
+  if (launch_zstd_decompress(Z, d->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  CUDA_TRY(cudaMemcpyAsync(d->h_lz_sizes.p, d->d_lz_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, d->stream));
+  if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged frames stop here
+  p1.resize(n_frames);
+  b1.resize(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + f * s1_cap; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
+  return CLDN_OK;
+}
+
+static int decode_batch_device_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
+                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities) {
+  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
+  for (size_t f = 0; f < n_frames; ++f) {
+    if (out_capacities[f] / std::max<uint32_t>(info.point_step, 1u) < n_points) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+  }
+  std::vector<const void*> p1;
+  std::vector<size_t> b1;
+  if (int rc = zstd_stage2_device(d, info, n_frames, payloads, payload_bytes, p1, b1)) return rc;
+  cldn_info_t plain = info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities);
+}
+
+// Host pointers, compression ZSTD: the payloads go up compressed, the device decompresses and decodes them, the points
+// come back (with the caller's padding bytes, like the uncompressed host path).
+static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
+                                  const size_t* payload_bytes, void* const* outs) {
+  size_t in_total = 0;
+  std::vector<size_t> in_off(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) {
+    in_off[f] = in_total;
+    in_total += (payload_bytes[f] + 255) & ~size_t(255);
+  }
+  if (int rc = d->d_in.reserve(in_total + 256)) return rc;
+  std::vector<const void*> din(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) {
+    din[f] = d->d_in.p + in_off[f];
+    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(d->d_in.p + in_off[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->stream));
+  }
+  std::vector<const void*> p1;
+  std::vector<size_t> b1;
+  if (int rc = zstd_stage2_device(d, info, n_frames, din.data(), payload_bytes, p1, b1)) return rc;
+  cldn_info_t plain = info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  if (int rc = decoder_update_plan(d, plain)) return rc;
+  const size_t out_need = static_cast<size_t>(info.width) * info.height * info.point_step;
+  const size_t out_stride = (out_need + 255) & ~size_t(255);
+  if (int rc = d->d_out.reserve(out_stride * n_frames + 256)) return rc;
+  std::vector<void*> dout(n_frames);
+  std::vector<size_t> caps(n_frames, out_need);
+  for (size_t f = 0; f < n_frames; ++f) {
+    dout[f] = d->d_out.p + out_stride * f;
+    // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
+    if (d->has_padding && out_need) CUDA_TRY(cudaMemcpyAsync(dout[f], outs[f], out_need, cudaMemcpyHostToDevice, d->stream));
+  }
+  if (int rc = decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), dout.data(), caps.data())) return rc;
+  for (size_t f = 0; f < n_frames; ++f) {
+    if (out_need) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], out_need, cudaMemcpyDeviceToHost, d->stream));
+  }
+  return check_device_error(d->stream, d->d_err.p, d->h_err.p);
+}
+
 static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t n_frames, const void* const* payloads,
                              const size_t* payload_bytes, void* const* outs, const size_t* out_capacities, int mem, int sync) {
   if (!d || !info || (n_frames && (!payloads || !payload_bytes || !outs || !out_capacities))) {
@@ -1223,6 +1373,8 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
   if (mem == CLDN_MEM_DEVICE) {
     if (info->compression_opt == CLDN_COMP_LZ4) {
       if (int rc = decode_batch_device_lz4(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) return rc;
+    } else if (info->compression_opt == CLDN_COMP_ZSTD) {
+      if (int rc = decode_batch_device_zstd(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) return rc;
     } else if (int rc = decode_batch_device(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) {
       return rc;
     }
@@ -1238,9 +1390,10 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
     }
   }
   if (info->compression_opt != CLDN_COMP_NONE) {
-    // stage 2 first (host libraries), then the ordinary stage-1 decode of the re-framed payload
+    // stage 2 first (ZSTD: on the device; LZ4: host library), then the ordinary stage-1 decode of the re-framed payload
     if (info->compression_opt > CLDN_COMP_ZSTD) { set_error("Unsupported compression option"); return CLDN_ERR_INVALID_ARGUMENT; }
-    if (!g_stage2.load(info->compression_opt)) return CLDN_ERR_UNSUPPORTED;
+    const bool device_zstd = info->compression_opt == CLDN_COMP_ZSTD && !zstd_host_route();
+    if (!device_zstd && !g_stage2.load(info->compression_opt)) return CLDN_ERR_UNSUPPORTED;
     cldn_info_t plain = *info;
     plain.compression_opt = CLDN_COMP_NONE;
     bool ok;
@@ -1251,9 +1404,9 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
         return CLDN_ERR_BUFFER_TOO_SMALL;
       }
     }
-    size_t max_body = max_compressed_size(plain, std::min<size_t>(pts, kChunkPoints), false, &ok);
+    const size_t max_body = stage2_max_body(*info, &ok);
     if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-    max_body = std::max<size_t>(max_body, pts * info->point_step) + 64;  // DecompressChunk's bound is w*h*step (cloudini.cpp:672-675)
+    if (device_zstd) return decode_batch_host_zstd(d, *info, n_frames, payloads, payload_bytes, outs);
     for (size_t f = 0; f < n_frames; ++f) {
       if (int rc = stage2_decompress_payload(info->compression_opt, static_cast<const uint8_t*>(payloads[f]), payload_bytes[f], d->s2_tmp, max_body)) return rc;
       const void* p1 = d->s2_tmp.data();

@@ -25,6 +25,7 @@ enum DevError : uint32_t {
   DEV_ERR_OUTPUT_SMALL = 10,
   DEV_ERR_LZ4 = 12,                  // "LZ4 decompression failed" codec_common.cpp:279-281
   DEV_ERR_ENCODE_OUTPUT_SMALL = 11,  // "Output buffer too small for uncompressed chunk" chunk_writer.cpp:33-35
+  DEV_ERR_ZSTD = 13,                 // "ZSTD decompression failed" codec_common.cpp:290-293
 };
 
 __device__ __forceinline__ void report_error(uint32_t* err, uint32_t code) { atomicCAS(err, 0u, code); }

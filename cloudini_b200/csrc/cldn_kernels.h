@@ -166,6 +166,23 @@ struct Lz4Launch {
 };
 int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
 int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream);
+// Re-frames the slots of L (chunk_sizes[] bytes each) into one stage-1 payload per frame at plain_out; a payload that
+// does not fit plain_cap raises `fail_code`.
+int launch_stage2_unpack(const Lz4Launch& L, uint32_t fail_code, cudaStream_t stream);
+
+// ---- ZSTD frames per chunk on the device (cldn_zstd.cu) ------------------------------------------------------------------
+// The chunk table, slots and frames are those of the LZ4 path (L.frames[f].packed_in: ([u32 csize][ZSTD frames])*).
+// Every chunk decompresses exactly as ZSTD_decompress(slot, body_cap, body, csize) does, failing exactly when it fails;
+// a failure raises DEV_ERR_ZSTD. A frame whose payload holds more chunks than n_chunks raises DEV_ERR_CHUNK_COUNT.
+struct ZstdLaunch {
+  Lz4Launch L;
+  uint32_t body_cap;       // bytes a chunk may decompress to (<= L.slot_stride)
+  uint32_t n_ctas;         // grid of the decompressor: warps walk the chunks with a grid stride
+  uint8_t* lit_scratch;    // n_ctas * zstd_warps_per_cta() regions of zstd_lit_scratch_bytes(body_cap) bytes
+};
+uint32_t zstd_warps_per_cta();
+size_t zstd_lit_scratch_bytes(uint32_t body_cap);
+int launch_zstd_decompress(const ZstdLaunch& Z, cudaStream_t stream);
 
 uint64_t kernel_launch_count();
 void count_launch(int n = 1);

@@ -23,6 +23,7 @@
 
 #include "cldn_device.cuh"
 #include "cldn_kernels.h"
+#include "cldn_stage2.cuh"
 
 namespace cldn {
 
@@ -38,52 +39,6 @@ constexpr int kLzMinMatch = CLDN_LZ4_MIN_MATCH;   // 4 (the format's minimum) ..
 //   5: 6.747 B per point    6: 6.797    8: 6.825 (the block framing outweighs the matches). Shorter minimum matches were
 // slower to encode and decode; 6 never expands and was close to 8 in time.
 
-__device__ __forceinline__ uint32_t lz_load32(const uint8_t* p) {  // any alignment
-  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
-  const uint32_t sh = static_cast<uint32_t>(a & 3u) * 8u;
-  if (sh == 0) return w[0];
-  return __funnelshift_r(w[0], w[1], sh);
-}
-__device__ __forceinline__ uint2 lz_load64(const uint8_t* p) {  // any alignment; reads the aligned words covering [p, p + 8)
-  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
-  const uint32_t sh = static_cast<uint32_t>(a & 3u) * 8u;
-  const uint32_t w0 = w[0], w1 = w[1];
-  if (sh == 0) return make_uint2(w0, w1);
-  const uint32_t w2 = w[2];
-  return make_uint2(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh));
-}
-// n bytes from src to dst by `nt` threads (this one is `tid`): 16-byte stores for the aligned body of dst, the (unaligned)
-// source through aligned words + funnel shifts. Reads the aligned words covering [src, src + n) only.
-__device__ __forceinline__ void lz_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, uint32_t tid, uint32_t nt) {
-  uint32_t head = (16u - static_cast<uint32_t>(reinterpret_cast<uintptr_t>(dst) & 15u)) & 15u;
-  if (head > n) head = n;
-  for (uint32_t k = tid; k < head; k += nt) dst[k] = src[k];
-  const uint32_t nv = (n - head) >> 4;
-  const uint8_t* s0 = src + head;
-  const uint32_t a = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(s0) & 3u);
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(s0 - a);
-  uint4* dv = reinterpret_cast<uint4*>(dst + head);
-  if (a == 0u) {
-    for (uint32_t v = tid; v < nv; v += nt) {
-      const uint32_t* q = w + 4u * v;
-      dv[v] = make_uint4(q[0], q[1], q[2], q[3]);
-    }
-  } else {
-    const uint32_t sh = a * 8u;
-    for (uint32_t v = tid; v < nv; v += nt) {
-      const uint32_t* q = w + 4u * v;
-      const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = q[4];
-      dv[v] = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
-    }
-  }
-  for (uint32_t k = head + (nv << 4) + tid; k < n; k += nt) dst[k] = src[k];
-}
-__device__ __forceinline__ void lz_prefetch(const void* p, bool l1) {
-  if (l1) asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
-  else asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
 __device__ __forceinline__ uint32_t lz_mix(uint32_t v) { return v * 2654435761u; }
 __device__ __forceinline__ uint32_t lz_slot(uint32_t m) { return m >> (32u - kLzHashBits); }           // top bits: the table slot
 __device__ __forceinline__ uint32_t lz_tag(uint32_t m) { return (m << kLzHashBits) & 0xFFFF0000u; }   // the 16 bits below them, moved to the entry's top half
@@ -252,19 +207,6 @@ __device__ uint32_t lz4_decompress_warp(const uint8_t* __restrict__ src, uint32_
   return op;
 }
 
-// Position of chunk `c` inside a framed payload ([u32 size][bytes])*: *body = offset of its bytes, returns its size;
-// 0xFFFFFFFF if the chain leaves the payload. (<= a few dozen hops: every frame has ceil(points / 32768) chunks.)
-__device__ __forceinline__ uint32_t lz_find_chunk(const uint8_t* payload, uint64_t bytes, uint32_t c, uint64_t* body) {
-  uint64_t pos = 0;
-  for (uint32_t k = 0;; ++k) {
-    if (bytes - pos < 4u || pos > bytes) return 0xFFFFFFFFu;
-    const uint32_t sz = load_u32(payload + pos);
-    if (sz > bytes - pos - 4u) return 0xFFFFFFFFu;
-    if (k == c) { *body = pos + 4u; return sz; }
-    pos += 4ull + sz;
-  }
-}
-
 // grid: ceil(n_chunks_total / 4) CTAs of 4 warps; warp -> (frame, chunk) through chunk_frame[]
 __global__ void __launch_bounds__(kLzThreads) lz4_compress_chunks_kernel(const Lz4Launch L) {
   __shared__ uint32_t s_table[kLzWarps][1u << kLzHashBits];
@@ -304,7 +246,9 @@ __global__ void __launch_bounds__(kLzThreads) lz4_decompress_chunks_kernel(const
 
 // One CTA per frame: ([u32 size][bytes])* of the frame's chunks, back to back at `dst` (behind `header_bytes` bytes of
 // header, which are copied too); the frame's total goes to sizes[f]. Stores are checked against dst_cap.
-__global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L, const uint8_t* header, uint32_t header_bytes, int to_blob) {
+// (shared by the ZSTD decompressor, launch_stage2_unpack: `unpack_err` is the code of a re-framed payload that does not fit)
+__global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L, const uint8_t* header, uint32_t header_bytes, int to_blob,
+                                                              uint32_t unpack_err) {
   const uint32_t f = blockIdx.x;
   const Lz4Frame F = L.frames[f];
   uint8_t* dst = to_blob ? F.blob_out : F.plain_out;
@@ -327,7 +271,7 @@ __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L,
   if (threadIdx.x == 0) {
     s_pos = pos;
     L.sizes[f] = fits ? pos : 0ull;
-    if (!fits) report_error(L.err, to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : DEV_ERR_LZ4);
+    if (!fits) report_error(L.err, to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : unpack_err);
   }
   (void)s_pos;
 }
@@ -339,7 +283,7 @@ int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t head
     lz4_compress_chunks_kernel<<<(L.n_chunks_total + kLzWarps - 1) / kLzWarps, kLzThreads, 0, stream>>>(L);
     ++n;
   }
-  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, header, header_bytes, 1);
+  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, header, header_bytes, 1, DEV_ERR_LZ4);
   count_launch(n + 1);
   return n + 1;
 }
@@ -351,9 +295,16 @@ int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream) {
     lz4_decompress_chunks_kernel<<<(L.n_chunks_total + kLzWarps - 1) / kLzWarps, kLzThreads, 0, stream>>>(L);
     ++n;
   }
-  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, nullptr, 0, 0);
+  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, nullptr, 0, 0, DEV_ERR_LZ4);
   count_launch(n + 1);
   return n + 1;
+}
+
+int launch_stage2_unpack(const Lz4Launch& L, uint32_t fail_code, cudaStream_t stream) {
+  if (L.n_frames == 0) return 0;
+  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, nullptr, 0, 0, fail_code);
+  count_launch(1);
+  return 1;
 }
 
 }  // namespace cldn

@@ -74,8 +74,9 @@ typedef struct cldn_info_t {
   uint32_t height;
   uint32_t point_step;
   uint8_t encoding_opt;    /* cldn_encoding_opt_t, default LOSSY */
-  uint8_t compression_opt; /* cldn_compression_opt_t. Stage 2 is not the product: NONE everywhere; LZ4/ZSTD only through the
-                              host-pointer API, where each chunk is handed to the system liblz4/libzstd (dlopen) */
+  uint8_t compression_opt; /* cldn_compression_opt_t. NONE everywhere. LZ4: both APIs (device kernels; the host-pointer
+                              API hands each chunk to the system liblz4). ZSTD: decode with both APIs on the device;
+                              encode through the host-pointer API only, each chunk handed to the system libzstd (dlopen) */
   uint8_t version;         /* wire version 2..5, default 5 */
   uint8_t use_threads;     /* accepted for API parity; ignored (there is no stage-2 worker thread here) */
   uint32_t n_fields;

@@ -6,6 +6,9 @@ runs this file in a child process with a timeout and records whatever JSON line 
   c3    BASELINE configs[2]: 1M-point XYZ + rgba u32 + ring u16 (V5 adaptive sections), 32 frames, encode / decode ms
   c4    BASELINE configs[3] with the Velodyne XYZIRT layout (step 22), 64 frames of 130 048 points, encode / decode ms
   msg   the DDS converter step (parse -> profile -> viz -> compress message) on one 1M-point PointCloud2, host buffers
+  zstd  the headline's 128 XYZI frames compressed once with ZSTD level 1 (what Cloudini ships, host-pointer encoder):
+        device-resident ZSTD + stage-1 decode per batch, one-message host-pointer decode latency, libzstd decompression
+        of the same chunks on one host core, bytes per point; parity with the oracle before any number
 """
 import json
 import os
@@ -202,9 +205,78 @@ def bench_msg(out):
                                      "(pooled handles); fused_*: cldn_b200_ros_convert_msg")
 
 
+def bench_zstd(out):
+    import ctypes as C
+    import struct
+    from oracle.client import best_oracle
+    F, n = 128, 1_000_000
+    info, _ = synth.cloud_c2(n, seed=1000)
+    info.compression_opt = cb.CompressionOption.ZSTD
+    enc = cb.PointcloudEncoder(info)
+    clouds = [synth.cloud_c2(n, seed=1000 + k)[1] for k in range(F)]   # the headline step's frames (bench.py)
+    blobs = [enc.encode(c) for c in clouds]
+    hdr = cb.DecodeHeader(blobs[0])[1]
+    s = torch.cuda.Stream()
+    torch.cuda.set_stream(s)
+    dec = cb.PointcloudDecoder(stream=s.cuda_stream)
+    d_in = [torch.from_numpy(np.frombuffer(b[hdr:], dtype=np.uint8).copy()).cuda() for b in blobs]
+    d_out = [torch.zeros(n * 16, dtype=torch.uint8, device="cuda") for _ in range(F)]
+    db = dec.make_device_batch([t.data_ptr() for t in d_in], [t.numel() for t in d_in], [t.data_ptr() for t in d_out], [n * 16] * F)
+    dec.decode_batch_device(info, db, sync=True)
+    # parity: the oracle's decode of the same blob (libzstd + stage 1), every 16th frame
+    oracle = best_oracle()
+    ok = True
+    for k in range(F):
+        if k % 16 == 0:
+            want = np.zeros(n * 16, dtype=np.uint8)
+            oracle.decode(blobs[k], want)
+            ok = ok and bool(np.array_equal(d_out[k].cpu().numpy(), want))
+    if not ok:
+        out["zstd_decode"] = {"parity": "MISMATCH against the oracle"}
+        return
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    for _ in range(2):
+        dec.decode_batch_device(info, db, sync=False)
+    reps, t = 5, 0.0
+    for _ in range(reps):
+        ev[0].record()
+        dec.decode_batch_device(info, db, sync=False)
+        ev[1].record()
+        torch.cuda.synchronize()
+        t += ev[0].elapsed_time(ev[1])
+    dev_ms = t / reps
+    host_dec = cb.PointcloudDecoder()
+    outbuf = np.zeros(n * 16, dtype=np.uint8)
+    host_dec.decode(info, blobs[0][hdr:], outbuf)
+    t0 = time.perf_counter()
+    for _ in range(5):
+        host_dec.decode(info, blobs[0][hdr:], outbuf)
+    host_ms = (time.perf_counter() - t0) / 5 * 1e3
+    z = C.CDLL("libzstd.so.1")
+    z.ZSTD_decompress.restype = C.c_size_t
+    z.ZSTD_decompress.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    chunks, pos, p0 = [], 0, blobs[0][hdr:]
+    while pos < len(p0):
+        (c,) = struct.unpack_from("<I", p0, pos)
+        chunks.append(p0[pos + 4:pos + 4 + c])
+        pos += 4 + c
+    dst = C.create_string_buffer(1 << 20)
+    stage1 = 0
+    t0 = time.perf_counter()
+    for _ in range(5):
+        stage1 = sum(z.ZSTD_decompress(dst, 1 << 20, c, len(c)) for c in chunks)
+    lib_ms = (time.perf_counter() - t0) / 5 * 1e3
+    zbytes = float(np.mean([len(b) - hdr for b in blobs]))
+    out["zstd_decode"] = {"frames": F, "points": n, "parity": f"bit-exact vs {oracle.kind} oracle (every 16th frame)",
+                          "zstd_B_per_pt": zbytes / n, "stage1_B_per_pt": stage1 / n,
+                          "device_batch_ms": dev_ms, "device_ms_per_frame": dev_ms / F, "device_mpts": F * n / dev_ms / 1e3,
+                          "host_api_one_message_ms": host_ms, "libzstd_one_core_ms_per_frame": lib_ms,
+                          "libzstd_one_core_mbs": stage1 / lib_ms / 1e3}
+
+
 if __name__ == "__main__":
     out = {}
-    for name, fn in (("viz", bench_viz), ("c3", bench_c3), ("c4", bench_c4_mixed), ("msg", bench_msg)):
+    for name, fn in (("viz", bench_viz), ("c3", bench_c3), ("c4", bench_c4_mixed), ("msg", bench_msg), ("zstd", bench_zstd)):
         try:
             fn(out)
         except Exception as e:  # noqa: BLE001 — an extra must never take the others down
