@@ -145,6 +145,11 @@ def lib():
     L.cldn_b200_decode.argtypes = [vp, C.POINTER(_CInfo), vp, sz, vp, sz, C.c_int]
     L.cldn_b200_decode_batch.argtypes = [vp, C.POINTER(_CInfo), sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp),
                                          C.POINTER(sz), C.c_int, C.c_int]
+    L.cldn_b200_decode_blobs.argtypes = [vp, sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.c_int,
+                                         C.POINTER(C.c_int32), C.POINTER(sz)]
+    L.cldn_b200_decoder_frame_error.argtypes = [vp, sz]
+    L.cldn_b200_decoder_frame_error.restype = C.c_char_p
+    L.cldn_b200_decoder_frame_info.argtypes = [vp, sz, C.POINTER(_CInfo)]
     L.cldn_b200_decoder_sync.argtypes = [vp]
     L.cldn_b200_decoder_last_stats.argtypes = [vp, C.POINTER(C.c_uint32)]
     L.cldn_b200_decoder_last_sections_ahead.argtypes = [vp]
@@ -398,6 +403,51 @@ class PointcloudDecoder:
         _check(lib().cldn_b200_decode_batch(self._h, C.byref(c), n, (C.c_void_p * n)(*[p[0] for p in ins]),
                                             (C.c_size_t * n)(*[p[1] for p in ins]), (C.c_void_p * n)(*[p[0] for p in outs]),
                                             (C.c_size_t * n)(*[p[1] for p in outs]), MEM_HOST, 1))
+
+    def _blobs(self, n, a_in, a_inb, a_out, a_cap, mem):
+        status = (C.c_int32 * max(n, 1))()
+        lib().cldn_b200_decode_blobs(self._h, n, a_in, a_inb, a_out, a_cap, mem, status, None)
+        infos = []
+        for f in range(n):
+            c = _CInfo()
+            _check(lib().cldn_b200_decoder_frame_info(self._h, f, C.byref(c)))
+            infos.append(_from_c(c) if c.version else None)  # zeroed where the header did not parse
+        return [int(status[f]) for f in range(n)], infos
+
+    def decode_blobs(self, blobs: Sequence, outputs: Optional[Sequence] = None):
+        """Complete blobs (header included, as encode() returns them) in any mix of layouts, point counts, wire versions
+        3..5 and compressions, host memory. Frames of one layout and compression are decoded together. Returns one
+        (status, EncodingInfo | None, output | None) per blob: status 0 or the negative cldn_status_t that DecodeHeader +
+        decode give that blob alone (its message: frame_error(f)); output is None for a failed frame. `outputs` (numpy
+        uint8, pre-filled) are decoded in place when given; only declared field bytes are overwritten."""
+        import numpy as np
+        n = len(blobs)
+        if outputs is None:
+            outputs = []
+            for b in blobs:
+                try:
+                    info, _ = DecodeHeader(b)
+                    outputs.append(np.zeros(info.width * info.height * info.point_step, dtype=np.uint8))
+                except (RuntimeError, MemoryError, ValueError):   # the decoder reports the frame's status
+                    outputs.append(np.zeros(0, dtype=np.uint8))
+        ins = [_host_ptr(b) for b in blobs]
+        outs = [_host_ptr(o) for o in outputs]
+        status, infos = self._blobs(n, (C.c_void_p * max(n, 1))(*[p[0] for p in ins]), (C.c_size_t * max(n, 1))(*[p[1] for p in ins]),
+                                    (C.c_void_p * max(n, 1))(*[p[0] for p in outs]), (C.c_size_t * max(n, 1))(*[p[1] for p in outs]),
+                                    MEM_HOST)
+        return [(status[f], infos[f], outputs[f] if status[f] == 0 else None) for f in range(n)]
+
+    def decode_blobs_device(self, ptrs: Sequence[int], sizes: Sequence[int], out_ptrs: Sequence[int], out_caps: Sequence[int]):
+        """decode_blobs for device-resident blobs and outputs (device addresses). Returns (statuses, EncodingInfos), an
+        info being None where the header did not parse."""
+        n = len(ptrs)
+        m = max(n, 1)
+        return self._blobs(n, (C.c_void_p * m)(*ptrs), (C.c_size_t * m)(*sizes), (C.c_void_p * m)(*out_ptrs),
+                           (C.c_size_t * m)(*out_caps), MEM_DEVICE)
+
+    def frame_error(self, f: int) -> str:
+        """Message of frame f of the last decode_blobs / decode_blobs_device ("" when it decoded)."""
+        return lib().cldn_b200_decoder_frame_error(self._h, f).decode("utf-8", "replace")
 
     def sync(self):
         _check(lib().cldn_b200_decoder_sync(self._h))

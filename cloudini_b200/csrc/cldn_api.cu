@@ -688,6 +688,7 @@ static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void*
   Z.chunk_sizes = e->d_lz_chunk_sizes.p;
   Z.sizes = e->d_sizes.p;   // the pack kernel overwrites the stage-1 sizes with the blob sizes (it runs after every reader)
   Z.err = e->d_err.p;
+  Z.frame_err = nullptr;
   if (launch_lz4_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) { set_error("LZ4 kernel launch failed"); return CLDN_ERR_CUDA; }
   CUDA_TRY(cudaGetLastError());
   return CLDN_OK;
@@ -874,6 +875,17 @@ struct cldn_decoder {
   bool sections_ahead = false;    // the last batch ran in side mode (cldn_b200_decoder_last_sections_ahead)
   CopyPipeline pipe;
   uint32_t epoch = 0;
+  // cldn_b200_decode_blobs: the first bytes of device-resident blobs, and what the last call found for every frame
+  DevBuf<uint64_t> d_blob_tab;
+  PinBuf<uint64_t> h_blob_tab;
+  DevBuf<uint8_t> d_prefix;
+  PinBuf<uint8_t> h_prefix;
+  // one error word per frame of the group being decoded (DecLaunch / Lz4Launch::frame_err); nullptr outside of it
+  DevBuf<uint32_t> d_frame_err;
+  PinBuf<uint32_t> h_frame_err;
+  uint32_t* frame_err = nullptr;
+  std::vector<std::string> frame_errors;
+  std::vector<cldn_info_t> frame_infos;
 };
 
 static bool same_info(const cldn_info_t& a, const cldn_info_t& b) {
@@ -927,19 +939,24 @@ static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
   return CLDN_OK;
 }
 
+// `frame_points` (optional): points of every frame; nullptr gives every frame info.width * info.height points.
 static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                               const size_t* payload_bytes, void* const* outs, const size_t* out_capacities) {
+                               const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
+                               const uint64_t* frame_points = nullptr) {
   d->sections_ahead = false;
   if (int rc = decoder_update_plan(d, info)) return rc;
-  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
-  if (n_points > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
-  const uint64_t out_need = n_points * info.point_step;
+  const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
+  for (size_t f = 0; f < (frame_points ? n_frames : 1); ++f) {
+    if ((frame_points ? frame_points[f] : wh) > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
+  }
   DecFrame* hf = nullptr;
   int hf_slot = 0;
   if (int rc = d->h_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
   if (int rc = d->d_frames.reserve(n_frames)) return rc;
   uint64_t chunks = 0;
   for (size_t f = 0; f < n_frames; ++f) {
+    const uint64_t n_points = frame_points ? frame_points[f] : wh;
+    const uint64_t out_need = n_points * info.point_step;
     if (out_capacities[f] < out_need) {
       set_error("Output buffer is too small to hold the decoded data");  // v4_codec.cpp:93-95 / v5_codec.cpp:991-993
       return CLDN_ERR_BUFFER_TOO_SMALL;
@@ -974,6 +991,7 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
   L.tile_capacity = 0; L.tile_grid = 0; L.epoch = 0; L.trace = nullptr; L.chunk_counter = nullptr; L.sections_only = 0;
   L.chunk_desc = nullptr; L.desc_tag = 0; L.uniform_chunks = 0; L.redo_list = nullptr; L.redo_mode = 0;
   L.side = nullptr; L.side_mode = 0;
+  L.frame_err = d->frame_err;
   for (int s = 0; s < kMaxSideFields; ++s) L.side_off[s] = 0;
   if (d->plan.n_sections > 0 && chunks > 0 && (d->plan.regular_overlap || !(d->plan.all_varint || d->plan.n_ops == 0))) {
     // V5 with raw / XOR / Gorilla fields in the regular stream: the per-chunk parser records where the sections start
@@ -1108,6 +1126,8 @@ void cldn_b200_decoder_destroy(cldn_decoder_t* d) {
   d->d_chunk_tiles.release(); d->d_chunk_tile_begin.release(); d->d_stream_end.release(); d->d_tsums.release(); d->d_tstatus.release(); d->d_chunk_frame.release(); d->d_tile_chunk.release(); d->d_trace.release(); d->d_counter.release(); d->d_redo.release(); d->d_side.release(); d->d_chunk_desc.release(); d->pipe.release();
   d->d_s1.release(); d->d_lz_scratch.release(); d->d_lz_chunk_frame.release(); d->d_lz_chunk_sizes.release(); d->d_lz_frames.release();
   d->d_lz_sizes.release(); d->h_lz_sizes.release(); d->h_lz_frames.release(); d->h_lz_chunk_frame.release(); d->d_zs_lit.release();
+  d->d_blob_tab.release(); d->h_blob_tab.release(); d->d_prefix.release(); d->h_prefix.release();
+  d->d_frame_err.release(); d->h_frame_err.release();
   if (d->own_stream && d->stream) cudaStreamDestroy(d->stream);
   delete d;
 }
@@ -1146,30 +1166,74 @@ int cldn_b200_decoder_last_sections_ahead(cldn_decoder_t* d) {
 
 }  // extern "C"
 
-static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                               const size_t* payload_bytes, void* const* outs, const size_t* out_capacities);
+// Points of every frame of a batch and where each frame's re-framed stage-1 payload goes in the decoder's arena:
+// `frame_points` as decode_batch_device takes it, every frame's chunks get a slot of `slot` bytes plus their u32 prefixes.
+struct FrameChunks {
+  std::vector<uint64_t> points;
+  std::vector<size_t> s1_off, s1_cap;
+  uint64_t max_points = 0;
+  size_t arena = 0, chunks = 0;
+  int init(const cldn_info_t& info, size_t n_frames, const uint64_t* frame_points) {
+    points.resize(n_frames);
+    for (size_t f = 0; f < n_frames; ++f) {
+      points[f] = frame_points ? frame_points[f] : static_cast<uint64_t>(info.width) * info.height;
+      if (points[f] > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
+      max_points = std::max(max_points, points[f]);
+    }
+    return CLDN_OK;
+  }
+  size_t frame_chunks(size_t f) const { return static_cast<size_t>((points[f] + kChunkPoints - 1) / kChunkPoints); }
+  void place(size_t slot) {
+    s1_off.resize(points.size());
+    s1_cap.resize(points.size());
+    for (size_t f = 0; f < points.size(); ++f) {
+      s1_cap[f] = (frame_chunks(f) * (slot + 4) + 255) & ~size_t(255);
+      s1_off[f] = arena;
+      arena += s1_cap[f];
+      chunks += frame_chunks(f);
+    }
+  }
+};
+
+// Frame and chunk tables of a stage-2 decompression launch (arena `s1`, laid out by FrameChunks::place).
+static void fill_stage2_frames(uint8_t* s1, const FrameChunks& fc, size_t n_frames, const void* const* payloads,
+                               const size_t* payload_bytes, Lz4Frame* hf, uint32_t* hcf) {
+  uint32_t cb = 0;
+  for (size_t f = 0; f < n_frames; ++f) {
+    Lz4Frame& F = hf[f];
+    memset(&F, 0, sizeof(F));
+    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
+    F.packed_in_bytes = payload_bytes[f];
+    F.plain_out = s1 + fc.s1_off[f];
+    F.plain_cap = fc.s1_cap[f];
+    F.n_chunks = static_cast<uint32_t>(fc.frame_chunks(f));
+    F.chunk_begin = cb;
+    for (uint32_t c = 0; c < F.n_chunks; ++c) hcf[cb + c] = static_cast<uint32_t>(f);
+    cb += F.n_chunks;
+  }
+}
 
 // Device pointers, compression LZ4: every chunk's block is decompressed on the device into a slot, the slots are re-framed
 // into a stage-1 payload per frame (internal arena) and the ordinary stage-1 decode runs on that. One read-back of the
 // frames' stage-1 sizes (8 bytes each) sits between the two.
 static int decode_batch_device_lz4(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                   const size_t* payload_bytes, void* const* outs, const size_t* out_capacities) {
+                                   const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
+                                   const uint64_t* frame_points = nullptr) {
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
-  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
-  if (n_points > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
+  FrameChunks fc;
+  if (int rc = fc.init(info, n_frames, frame_points)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
-    if (out_capacities[f] < n_points * info.point_step) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+    if (out_capacities[f] < fc.points[f] * info.point_step) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
   }
   bool ok;
-  const size_t chunks_per_frame = static_cast<size_t>((n_points + kChunkPoints - 1) / kChunkPoints);
-  const size_t max_chunk = max_compressed_size(plain, std::min<size_t>(n_points, kChunkPoints), false, &ok) + 64;
+  const size_t max_chunk = max_compressed_size(plain, std::min<size_t>(fc.max_points, kChunkPoints), false, &ok) + 64;
   if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
   const size_t slot = (max_chunk + 15) & ~size_t(15);
-  const size_t s1_cap = ((chunks_per_frame * (slot + 4) + 255) & ~size_t(255));
-  const size_t chunks = chunks_per_frame * n_frames;
+  fc.place(slot);
+  const size_t chunks = fc.chunks;
   if (chunks > 0x7FFFFFFFull || slot > 0xFFFFFFF0ull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = d->d_s1.reserve(std::max<size_t>(s1_cap * n_frames, 256))) return rc;
+  if (int rc = d->d_s1.reserve(std::max<size_t>(fc.arena, 256))) return rc;
   if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
   if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
   if (int rc = d->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
@@ -1180,17 +1244,7 @@ static int decode_batch_device_lz4(cldn_decoder* d, const cldn_info_t& info, siz
   uint32_t* hcf = nullptr; int hcf_slot = 0;
   if (int rc = d->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
   if (int rc = d->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) {
-    Lz4Frame& F = hf[f];
-    memset(&F, 0, sizeof(F));
-    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
-    F.packed_in_bytes = payload_bytes[f];
-    F.plain_out = d->d_s1.p + f * s1_cap;
-    F.plain_cap = s1_cap;
-    F.n_chunks = static_cast<uint32_t>(chunks_per_frame);
-    F.chunk_begin = static_cast<uint32_t>(f * chunks_per_frame);
-    for (size_t c = 0; c < chunks_per_frame; ++c) hcf[f * chunks_per_frame + c] = static_cast<uint32_t>(f);
-  }
+  fill_stage2_frames(d->d_s1.p, fc, n_frames, payloads, payload_bytes, hf, hcf);
   CUDA_TRY(cudaMemcpyAsync(d->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_lz_frames.commit(hf_slot, d->stream)) return rc;
   if (chunks) CUDA_TRY(cudaMemcpyAsync(d->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
@@ -1205,22 +1259,22 @@ static int decode_batch_device_lz4(cldn_decoder* d, const cldn_info_t& info, siz
   Z.chunk_sizes = d->d_lz_chunk_sizes.p;
   Z.sizes = d->d_lz_sizes.p;
   Z.err = d->d_err.p;
+  Z.frame_err = d->frame_err;
   if (launch_lz4_decompress(Z, d->stream) < 0) { set_error("LZ4 kernel launch failed"); return CLDN_ERR_CUDA; }
   CUDA_TRY(cudaMemcpyAsync(d->h_lz_sizes.p, d->d_lz_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, d->stream));
   if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged blocks stop here
   std::vector<const void*> p1(n_frames);
   std::vector<size_t> b1(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + f * s1_cap; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
-  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities);
+  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + fc.s1_off[f]; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
+  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities, frame_points);
 }
 
 // Bound of one decompressed chunk, as the host-pointer API has always passed it to ZSTD_decompress / LZ4_decompress_safe:
 // the stage-1 worst case of a chunk, or the whole frame's bytes if larger (DecompressChunk's bound is w*h*step,
 // cloudini.cpp:672-675), plus 64.
-static size_t stage2_max_body(const cldn_info_t& info, bool* ok) {
+static size_t stage2_max_body(const cldn_info_t& info, size_t pts, bool* ok) {
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
-  const size_t pts = static_cast<size_t>(info.width) * info.height;
   const size_t m = max_compressed_size(plain, std::min<size_t>(pts, kChunkPoints), false, ok);
   return std::max<size_t>(m, pts * info.point_step) + 64;
 }
@@ -1236,30 +1290,30 @@ static bool zstd_host_route() {
 // of cldn_zstd.cu. A chunk may decompress to max_body bytes (the host-pointer bound) but not beyond its slot, which holds
 // the stage-1 worst case of a 32768-point chunk: a larger chunk body cannot be a stage-1 chunk and is refused as damaged.
 // On return p1 / b1 are the frames' stage-1 payloads in the internal arena (one read-back of their sizes).
+// `frame_points` as decode_batch_device takes it: the frames of one launch share one chunk bound (that of the largest).
 static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads, const size_t* payload_bytes,
-                              std::vector<const void*>& p1, std::vector<size_t>& b1) {
+                              std::vector<const void*>& p1, std::vector<size_t>& b1, const uint64_t* frame_points = nullptr) {
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
-  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
-  if (n_points > 0xFFFFFFFFull) { set_error("too many points"); return CLDN_ERR_UNSUPPORTED; }
+  FrameChunks fc;
+  if (int rc = fc.init(info, n_frames, frame_points)) return rc;
   bool ok;
-  const size_t max_body = stage2_max_body(info, &ok);
+  const size_t max_body = stage2_max_body(info, fc.max_points, &ok);
   if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-  const size_t chunks_per_frame = static_cast<size_t>((n_points + kChunkPoints - 1) / kChunkPoints);
-  const size_t chunk_worst = max_compressed_size(plain, std::min<size_t>(n_points, kChunkPoints), false, &ok) + 64;
+  const size_t chunk_worst = max_compressed_size(plain, std::min<size_t>(fc.max_points, kChunkPoints), false, &ok) + 64;
   const size_t cap = std::min(max_body, chunk_worst);
   const size_t slot = (cap + 15) & ~size_t(15);
-  const size_t s1_cap = ((chunks_per_frame * (slot + 4) + 255) & ~size_t(255));
-  const size_t chunks = chunks_per_frame * n_frames;
+  fc.place(slot);
+  const size_t chunks = fc.chunks;
   if (chunks > 0x7FFFFFFFull || slot > 0xFFFFFFF0ull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
   for (size_t f = 0; f < n_frames; ++f) {  // a frame without points has no chunk to decompress
-    if (chunks_per_frame == 0 && payload_bytes[f] != 0) { set_error("%s", dev_error_text(DEV_ERR_CHUNK_COUNT)); return CLDN_ERR_CORRUPT_DATA; }
+    if (fc.frame_chunks(f) == 0 && payload_bytes[f] != 0) { set_error("%s", dev_error_text(DEV_ERR_CHUNK_COUNT)); return CLDN_ERR_CORRUPT_DATA; }
   }
   // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
   const uint32_t wpc = zstd_warps_per_cta();
   const size_t ctas = std::max<size_t>(1, std::min<size_t>((chunks + wpc - 1) / wpc, 2048 / wpc));
   const size_t lit_stride = zstd_lit_scratch_bytes(static_cast<uint32_t>(cap));
-  if (int rc = d->d_s1.reserve(std::max<size_t>(s1_cap * n_frames, 256))) return rc;
+  if (int rc = d->d_s1.reserve(std::max<size_t>(fc.arena, 256))) return rc;
   if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
   if (int rc = d->d_zs_lit.reserve(ctas * wpc * lit_stride)) return rc;
   if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
@@ -1271,17 +1325,7 @@ static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n
   uint32_t* hcf = nullptr; int hcf_slot = 0;
   if (int rc = d->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
   if (int rc = d->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) {
-    Lz4Frame& F = hf[f];
-    memset(&F, 0, sizeof(F));
-    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
-    F.packed_in_bytes = payload_bytes[f];
-    F.plain_out = d->d_s1.p + f * s1_cap;
-    F.plain_cap = s1_cap;
-    F.n_chunks = static_cast<uint32_t>(chunks_per_frame);
-    F.chunk_begin = static_cast<uint32_t>(f * chunks_per_frame);
-    for (size_t c = 0; c < chunks_per_frame; ++c) hcf[f * chunks_per_frame + c] = static_cast<uint32_t>(f);
-  }
+  fill_stage2_frames(d->d_s1.p, fc, n_frames, payloads, payload_bytes, hf, hcf);
   CUDA_TRY(cudaMemcpyAsync(d->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_lz_frames.commit(hf_slot, d->stream)) return rc;
   if (chunks) CUDA_TRY(cudaMemcpyAsync(d->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
@@ -1297,6 +1341,7 @@ static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n
   Z.L.chunk_sizes = d->d_lz_chunk_sizes.p;
   Z.L.sizes = d->d_lz_sizes.p;
   Z.L.err = d->d_err.p;
+  Z.L.frame_err = d->frame_err;
   Z.body_cap = static_cast<uint32_t>(cap);
   Z.n_ctas = static_cast<uint32_t>(ctas);
   Z.lit_scratch = d->d_zs_lit.p;
@@ -1305,28 +1350,30 @@ static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n
   if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged frames stop here
   p1.resize(n_frames);
   b1.resize(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + f * s1_cap; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
+  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + fc.s1_off[f]; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
   return CLDN_OK;
 }
 
 static int decode_batch_device_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities) {
-  const uint64_t n_points = static_cast<uint64_t>(info.width) * info.height;
+                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
+                                    const uint64_t* frame_points = nullptr) {
+  const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
   for (size_t f = 0; f < n_frames; ++f) {
+    const uint64_t n_points = frame_points ? frame_points[f] : wh;
     if (out_capacities[f] / std::max<uint32_t>(info.point_step, 1u) < n_points) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
   }
   std::vector<const void*> p1;
   std::vector<size_t> b1;
-  if (int rc = zstd_stage2_device(d, info, n_frames, payloads, payload_bytes, p1, b1)) return rc;
+  if (int rc = zstd_stage2_device(d, info, n_frames, payloads, payload_bytes, p1, b1, frame_points)) return rc;
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
-  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities);
+  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities, frame_points);
 }
 
 // Host pointers, compression ZSTD: the payloads go up compressed, the device decompresses and decodes them, the points
 // come back (with the caller's padding bytes, like the uncompressed host path).
 static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                  const size_t* payload_bytes, void* const* outs) {
+                                  const size_t* payload_bytes, void* const* outs, const uint64_t* frame_points = nullptr) {
   size_t in_total = 0;
   std::vector<size_t> in_off(n_frames);
   for (size_t f = 0; f < n_frames; ++f) {
@@ -1341,24 +1388,72 @@ static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size
   }
   std::vector<const void*> p1;
   std::vector<size_t> b1;
-  if (int rc = zstd_stage2_device(d, info, n_frames, din.data(), payload_bytes, p1, b1)) return rc;
+  if (int rc = zstd_stage2_device(d, info, n_frames, din.data(), payload_bytes, p1, b1, frame_points)) return rc;
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
   if (int rc = decoder_update_plan(d, plain)) return rc;
-  const size_t out_need = static_cast<size_t>(info.width) * info.height * info.point_step;
-  const size_t out_stride = (out_need + 255) & ~size_t(255);
-  if (int rc = d->d_out.reserve(out_stride * n_frames + 256)) return rc;
+  const size_t wh = static_cast<size_t>(info.width) * info.height;
+  std::vector<size_t> caps(n_frames), out_off(n_frames);
+  size_t out_total = 0;
+  for (size_t f = 0; f < n_frames; ++f) {
+    caps[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
+    out_off[f] = out_total;
+    out_total += (caps[f] + 255) & ~size_t(255);
+  }
+  if (int rc = d->d_out.reserve(out_total + 256)) return rc;
   std::vector<void*> dout(n_frames);
-  std::vector<size_t> caps(n_frames, out_need);
   for (size_t f = 0; f < n_frames; ++f) {
-    dout[f] = d->d_out.p + out_stride * f;
+    dout[f] = d->d_out.p + out_off[f];
     // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
-    if (d->has_padding && out_need) CUDA_TRY(cudaMemcpyAsync(dout[f], outs[f], out_need, cudaMemcpyHostToDevice, d->stream));
+    if (d->has_padding && caps[f]) CUDA_TRY(cudaMemcpyAsync(dout[f], outs[f], caps[f], cudaMemcpyHostToDevice, d->stream));
   }
-  if (int rc = decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), dout.data(), caps.data())) return rc;
+  if (int rc = decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), dout.data(), caps.data(), frame_points)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
-    if (out_need) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], out_need, cudaMemcpyDeviceToHost, d->stream));
+    if (caps[f]) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], caps[f], cudaMemcpyDeviceToHost, d->stream));
   }
+  return check_device_error(d->stream, d->d_err.p, d->h_err.p);
+}
+
+// Host pointers, no stage 2. `frame_points` as decode_batch_device takes it.
+static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
+                                   const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
+                                   const uint64_t* frame_points = nullptr) {
+  if (int rc = decoder_update_plan(d, info)) return rc;
+  const size_t wh = static_cast<size_t>(info.width) * info.height;
+  size_t in_total = 0, out_total = 0;
+  std::vector<size_t> in_off(n_frames), out_need(n_frames), out_off(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) {
+    out_need[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
+    if (out_capacities[f] < out_need[f]) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+    in_off[f] = in_total;
+    in_total += (payload_bytes[f] + 255) & ~size_t(255);
+    out_off[f] = out_total;
+    out_total += (out_need[f] + 255) & ~size_t(255);
+  }
+  if (int rc = d->d_in.reserve(in_total + 256)) return rc;
+  if (int rc = d->d_out.reserve(out_total + 256)) return rc;
+  if (int rc = d->pipe.ensure(2 * n_frames)) return rc;
+  // frame f: upload on the h2d stream -> decode on the handle's stream -> download on the d2h stream
+  for (size_t f = 0; f < n_frames; ++f) {
+    const void* din = d->d_in.p + in_off[f];
+    void* dout = d->d_out.p + out_off[f];
+    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(d->d_in.p + in_off[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->pipe.h2d));
+    // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
+    if (d->has_padding && out_need[f]) CUDA_TRY(cudaMemcpyAsync(dout, outs[f], out_need[f], cudaMemcpyHostToDevice, d->pipe.h2d));
+    CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f], d->pipe.h2d));
+    CUDA_TRY(cudaStreamWaitEvent(d->stream, d->pipe.ev[2 * f], 0));
+    const uint64_t* pts = frame_points ? frame_points + f : nullptr;
+    uint32_t* const group_err = d->frame_err;
+    if (group_err) d->frame_err = group_err + f;  // one launch per frame: frame 0 of that launch is frame f of the group
+    const int rc = decode_batch_device(d, info, 1, &din, &payload_bytes[f], &dout, &out_need[f], pts);
+    d->frame_err = group_err;
+    if (rc) return rc;
+    CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f + 1], d->stream));
+    CUDA_TRY(cudaStreamWaitEvent(d->pipe.d2h, d->pipe.ev[2 * f + 1], 0));
+    if (out_need[f]) CUDA_TRY(cudaMemcpyAsync(outs[f], dout, out_need[f], cudaMemcpyDeviceToHost, d->pipe.d2h));
+  }
+  CUDA_TRY(cudaStreamSynchronize(d->pipe.d2h));
+  // a failed decode must not hand back garbage silently: the error word is checked after everything has drained
   return check_device_error(d->stream, d->d_err.p, d->h_err.p);
 }
 
@@ -1404,7 +1499,7 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
         return CLDN_ERR_BUFFER_TOO_SMALL;
       }
     }
-    const size_t max_body = stage2_max_body(*info, &ok);
+    const size_t max_body = stage2_max_body(*info, pts, &ok);
     if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
     if (device_zstd) return decode_batch_host_zstd(d, *info, n_frames, payloads, payload_bytes, outs);
     for (size_t f = 0; f < n_frames; ++f) {
@@ -1415,36 +1510,230 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
     }
     return CLDN_OK;
   }
-  if (int rc = decoder_update_plan(d, *info)) return rc;
-  const size_t out_need = static_cast<size_t>(info->width) * info->height * info->point_step;
-  size_t in_total = 0;
-  std::vector<size_t> in_off(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) {
-    if (out_capacities[f] < out_need) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-    in_off[f] = in_total;
-    in_total += (payload_bytes[f] + 255) & ~size_t(255);
+  return decode_batch_host_plain(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities);
+}
+
+// ---- complete blobs, any mix of layouts and sizes (cldn_b200_decode_blobs) -----------------------------------------
+constexpr size_t kBlobPrefix = 4096;  // bytes of every device-resident blob fetched for its header
+
+// Whether a header whose first `len` bytes are at p may parse once more of the blob is read: a YAML header with no NUL
+// yet, a binary header whose fields run past `len`. *want: bytes that would settle it, where the binary layout says so.
+static bool header_runs_past(const uint8_t* p, size_t len, size_t* want) {
+  *want = 0;
+  if (len < 12 || memcmp(p, "CLOUDINI_V", 10) != 0) return false;
+  auto digit = [](uint8_t c) -> int { return (c >= '0' && c <= '9') ? c - '0' : 0; };
+  const int version = digit(p[10]) * 10 + digit(p[11]);
+  if (version < 2 || version > CLDN_ENCODING_VERSION) return false;  // refused whatever follows
+  if (len < 14) return true;
+  if (p[12] == '\n' && p[13] != '{') return memchr(p + 13, 0, len - 13) == nullptr;
+  size_t pos = 12 + 14;  // binary layout of cldn_b200_decode_header: width, height, point_step, options, field count
+  if (len < pos) { *want = pos; return true; }
+  uint16_t nf;
+  memcpy(&nf, p + pos - 2, 2);
+  if (nf > CLDN_MAX_FIELDS) return false;
+  for (uint16_t i = 0; i < nf; ++i) {
+    if (len < pos + 2) { *want = pos + 2; return true; }
+    uint16_t nl;
+    memcpy(&nl, p + pos, 2);
+    pos += 2 + nl + 9;
+    if (len < pos) { *want = pos; return true; }
   }
-  const size_t out_stride = (out_need + 255) & ~size_t(255);
-  if (int rc = d->d_in.reserve(in_total + 256)) return rc;
-  if (int rc = d->d_out.reserve(out_stride * n_frames + 256)) return rc;
-  if (int rc = d->pipe.ensure(2 * n_frames)) return rc;
-  // frame f: upload on the h2d stream -> decode on the handle's stream -> download on the d2h stream
-  for (size_t f = 0; f < n_frames; ++f) {
-    const void* din = d->d_in.p + in_off[f];
-    void* dout = d->d_out.p + out_stride * f;
-    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(d->d_in.p + in_off[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->pipe.h2d));
-    // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
-    if (d->has_padding && out_need) CUDA_TRY(cudaMemcpyAsync(dout, outs[f], out_need, cudaMemcpyHostToDevice, d->pipe.h2d));
-    CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f], d->pipe.h2d));
-    CUDA_TRY(cudaStreamWaitEvent(d->stream, d->pipe.ev[2 * f], 0));
-    if (int rc = decode_batch_device(d, *info, 1, &din, &payload_bytes[f], &dout, &out_need)) return rc;
-    CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f + 1], d->stream));
-    CUDA_TRY(cudaStreamWaitEvent(d->pipe.d2h, d->pipe.ev[2 * f + 1], 0));
-    if (out_need) CUDA_TRY(cudaMemcpyAsync(outs[f], dout, out_need, cudaMemcpyDeviceToHost, d->pipe.d2h));
+  return false;
+}
+
+// Headers of every blob, parsed by cldn_b200_decode_header: in place for host memory. Device blobs: one launch gathers
+// the first min(blob_bytes, kBlobPrefix) bytes of every blob, packed back to back, behind one read-back and one
+// synchronisation; a header that runs past its prefix is read again, twice as long each time (or as long as its binary
+// layout says), until it parses or the blob ends, so every frame gets the status its complete header gives.
+static int read_blob_headers(cldn_decoder* d, size_t n, const void* const* blobs, const size_t* blob_bytes, int mem,
+                             std::vector<size_t>& hdr, int32_t* status) {
+  hdr.assign(n, 0);
+  auto parse = [&](size_t f, const uint8_t* p, size_t len) {
+    status[f] = cldn_b200_decode_header(p, len, &d->frame_infos[f], &hdr[f]);
+    d->frame_errors[f] = status[f] == CLDN_OK ? "" : cldn_b200_last_error();
+    if (status[f] != CLDN_OK) d->frame_infos[f] = cldn_info_t{};
+  };
+  if (mem == CLDN_MEM_HOST) {
+    for (size_t f = 0; f < n; ++f) parse(f, static_cast<const uint8_t*>(blobs[f]), blob_bytes[f]);
+    return CLDN_OK;
   }
-  CUDA_TRY(cudaStreamSynchronize(d->pipe.d2h));
-  // a failed decode must not hand back garbage silently: the error word is checked after everything has drained
-  return check_device_error(d->stream, d->d_err.p, d->h_err.p);
+  if (n > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
+  if (int rc = d->h_blob_tab.reserve(3 * n)) return rc;
+  if (int rc = d->d_blob_tab.reserve(3 * n)) return rc;
+  uint64_t* tab = d->h_blob_tab.p;
+  size_t total = 0;
+  for (size_t f = 0; f < n; ++f) {
+    tab[f] = reinterpret_cast<uint64_t>(blobs[f]);
+    tab[n + f] = blobs[f] ? std::min(blob_bytes[f], kBlobPrefix) : 0;
+    tab[2 * n + f] = total;
+    total += (tab[n + f] + 15) & ~size_t(15);
+  }
+  if (int rc = d->h_prefix.reserve(total + 16)) return rc;
+  if (int rc = d->d_prefix.reserve(total + 16)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(d->d_blob_tab.p, tab, 3 * n * sizeof(uint64_t), cudaMemcpyHostToDevice, d->stream));
+  if (launch_gather_prefixes(d->d_blob_tab.p, static_cast<uint32_t>(n), d->d_prefix.p, d->stream) < 0) { set_error("header gather launch failed"); return CLDN_ERR_CUDA; }
+  CUDA_TRY(cudaGetLastError());
+  if (total) CUDA_TRY(cudaMemcpyAsync(d->h_prefix.p, d->d_prefix.p, total, cudaMemcpyDeviceToHost, d->stream));
+  CUDA_TRY(cudaStreamSynchronize(d->stream));
+  std::vector<uint8_t> more;
+  for (size_t f = 0; f < n; ++f) {
+    if (!blobs[f]) { parse(f, nullptr, blob_bytes[f]); continue; }
+    const uint8_t* p = d->h_prefix.p + tab[2 * n + f];
+    size_t got = static_cast<size_t>(tab[n + f]), want = 0;
+    while (got < blob_bytes[f] && header_runs_past(p, got, &want)) {
+      got = std::min(blob_bytes[f], std::max(2 * got, want));
+      more.resize(got);
+      CUDA_TRY(cudaMemcpyAsync(more.data(), blobs[f], got, cudaMemcpyDeviceToHost, d->stream));
+      CUDA_TRY(cudaStreamSynchronize(d->stream));
+      p = more.data();
+    }
+    parse(f, p, got);
+  }
+  return CLDN_OK;
+}
+
+// Frames decoded by one fused launch: the same layout (width and height aside) and compression. LZ4 and ZSTD frames also
+// share the bound of a decompressed chunk, which depends on the points of a chunk, so that every frame is bounded
+// exactly as cldn_b200_decode bounds it.
+static bool same_group(const cldn_info_t& a, uint64_t a_points, const cldn_info_t& b, uint64_t b_points) {
+  cldn_info_t x = a, y = b;
+  x.width = y.width = x.height = y.height = 0;
+  if (!same_info(x, y) || strncmp(a.encoding_config, b.encoding_config, sizeof(a.encoding_config)) != 0) return false;
+  for (uint32_t i = 0; i < a.n_fields; ++i) {
+    if (strncmp(a.fields[i].name, b.fields[i].name, CLDN_MAX_NAME) != 0) return false;
+  }
+  return a.compression_opt == CLDN_COMP_NONE || std::min<uint64_t>(a_points, kChunkPoints) == std::min<uint64_t>(b_points, kChunkPoints);
+}
+
+// One group, synchronously, with an error word per frame (DecLaunch / Lz4Launch::frame_err). Device memory: one fused
+// stage-1 launch (behind one stage-2 launch for LZ4 / ZSTD). Host memory: the staging of cldn_b200_decode_batch.
+// frame_word[i] != 0: member i failed. A non-OK return (a CUDA error, a refused group, or an error no frame claimed)
+// says nothing about any single member.
+static int decode_blob_group(cldn_decoder* d, int mem, const cldn_info_t& info, size_t n, const void* const* payloads,
+                             const size_t* payload_bytes, void* const* outs, const size_t* caps, const uint64_t* points,
+                             std::vector<uint32_t>& frame_word) {
+  if (int rc = d->d_frame_err.reserve(n)) return rc;
+  if (int rc = d->h_frame_err.reserve(n)) return rc;
+  CUDA_TRY(cudaMemsetAsync(d->d_frame_err.p, 0, n * sizeof(uint32_t), d->stream));
+  d->frame_err = d->d_frame_err.p;
+  const int rc = [&]() -> int {
+    if (mem == CLDN_MEM_HOST) {
+      if (info.compression_opt == CLDN_COMP_ZSTD) return decode_batch_host_zstd(d, info, n, payloads, payload_bytes, outs, points);
+      return decode_batch_host_plain(d, info, n, payloads, payload_bytes, outs, caps, points);
+    }
+    int r;
+    if (info.compression_opt == CLDN_COMP_LZ4) r = decode_batch_device_lz4(d, info, n, payloads, payload_bytes, outs, caps, points);
+    else if (info.compression_opt == CLDN_COMP_ZSTD) r = decode_batch_device_zstd(d, info, n, payloads, payload_bytes, outs, caps, points);
+    else r = decode_batch_device(d, info, n, payloads, payload_bytes, outs, caps, points);
+    if (r) return r;
+    return check_device_error(d->stream, d->d_err.p, d->h_err.p);  // the launch word: errors no frame claimed
+  }();
+  d->frame_err = nullptr;
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(d->h_frame_err.p, d->d_frame_err.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, d->stream));
+  CUDA_TRY(cudaStreamSynchronize(d->stream));
+  frame_word.assign(d->h_frame_err.p, d->h_frame_err.p + n);
+  return CLDN_OK;
+}
+
+// Every frame ends with the status cldn_b200_decode_header + cldn_b200_decode give it alone. Frames go through their
+// group's fused launch, whose per-frame error words say which frames failed; only those are decoded again alone, which
+// gives them exactly the single-blob status and message (the kernels report the first defect they meet, the reference
+// the first in stream order). A group that fails as a whole (an error no frame claimed, a refused plan) has all its
+// frames decoded alone. Frames that the single-frame path handles frame by frame anyway (LZ4 with host pointers,
+// CLDN_B200_ZSTD_HOST) or refuses before any launch also take it directly.
+static int decode_blobs_impl(cldn_decoder* d, size_t n, const void* const* blobs, const size_t* blob_bytes, void* const* outs,
+                             const size_t* caps, int mem, int32_t* status, size_t* decoded_bytes) {
+  if (!d || (n && !status)) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  d->frame_errors.assign(n, "frame not decoded");
+  d->frame_infos.assign(n, cldn_info_t{});
+  for (size_t f = 0; f < n; ++f) {
+    status[f] = CLDN_ERR_INTERNAL;
+    if (decoded_bytes) decoded_bytes[f] = 0;
+  }
+  auto result = [&]() -> int {
+    for (size_t f = 0; f < n; ++f) {
+      if (status[f] != CLDN_OK) { set_error("frame %zu: %s", f, d->frame_errors[f].c_str()); return status[f]; }
+    }
+    return CLDN_OK;
+  };
+  auto fail_all = [&](int rc) {
+    const std::string msg = cldn_b200_last_error();
+    for (size_t f = 0; f < n; ++f) { status[f] = rc; d->frame_errors[f] = msg; }
+    return result();
+  };
+  if (n == 0) return CLDN_OK;
+  if (!blobs || !blob_bytes || !outs || !caps) { set_error("null argument"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE) { set_error("bad mem kind"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
+  if (cudaSetDevice(d->device) != cudaSuccess) { set_error("cudaSetDevice failed"); return fail_all(CLDN_ERR_CUDA); }
+  std::vector<size_t> hdr;
+  if (int rc = read_blob_headers(d, n, blobs, blob_bytes, mem, hdr, status)) return fail_all(rc);
+
+  std::vector<const void*> payload(n);
+  std::vector<size_t> payload_bytes(n);
+  std::vector<uint64_t> points(n);
+  std::vector<uint8_t> todo(n), alone(n);
+  for (size_t f = 0; f < n; ++f) {
+    if (status[f] != CLDN_OK) continue;
+    const cldn_info_t& I = d->frame_infos[f];
+    todo[f] = 1;
+    payload[f] = static_cast<const uint8_t*>(blobs[f]) + hdr[f];
+    payload_bytes[f] = blob_bytes[f] - hdr[f];
+    points[f] = static_cast<uint64_t>(I.width) * I.height;
+    alone[f] = I.version < 3 || I.compression_opt > CLDN_COMP_ZSTD || points[f] > 0xFFFFFFFFull || points[f] * I.point_step > caps[f];
+    if (mem == CLDN_MEM_HOST) {
+      alone[f] |= I.compression_opt == CLDN_COMP_LZ4 || (I.compression_opt == CLDN_COMP_ZSTD && zstd_host_route()) ||
+                  (payload_bytes[f] >= 10 && memcmp(payload[f], "CLOUDINI_V", 10) == 0);
+    }
+  }
+  std::vector<size_t> members;
+  std::vector<const void*> g_payload;
+  std::vector<size_t> g_bytes, g_caps;
+  std::vector<void*> g_outs;
+  std::vector<uint64_t> g_points;
+  std::vector<uint32_t> g_word;
+  for (size_t f = 0; f < n; ++f) {
+    if (!todo[f] || alone[f]) continue;
+    members.clear();
+    for (size_t g = f; g < n; ++g) {
+      if (todo[g] && !alone[g] && same_group(d->frame_infos[f], points[f], d->frame_infos[g], points[g])) {
+        members.push_back(g);
+        todo[g] = 0;
+      }
+    }
+    g_payload.clear(); g_bytes.clear(); g_caps.clear(); g_outs.clear(); g_points.clear();
+    for (size_t g : members) {
+      g_payload.push_back(payload[g]);
+      g_bytes.push_back(payload_bytes[g]);
+      g_outs.push_back(outs[g]);
+      g_caps.push_back(caps[g]);
+      g_points.push_back(points[g]);
+    }
+    // every member has its own point count: the group's info carries none, so that the decoder's cached plan (keyed by
+    // the whole info) survives from call to call whatever the frames' sizes
+    cldn_info_t layout = d->frame_infos[f];
+    layout.width = layout.height = 0;
+    const int rc = decode_blob_group(d, mem, layout, members.size(), g_payload.data(), g_bytes.data(), g_outs.data(),
+                                     g_caps.data(), g_points.data(), g_word);
+    for (size_t i = 0; i < members.size(); ++i) {
+      const size_t g = members[i];
+      if (rc != CLDN_OK || g_word[i] != 0) {
+        todo[g] = 1;
+        alone[g] = 1;
+        continue;
+      }
+      status[g] = CLDN_OK;
+      d->frame_errors[g].clear();
+      if (decoded_bytes) decoded_bytes[g] = static_cast<size_t>(points[g] * d->frame_infos[g].point_step);
+    }
+  }
+  for (size_t f = 0; f < n; ++f) {
+    if (!todo[f]) continue;
+    status[f] = decode_batch_impl(d, &d->frame_infos[f], 1, &payload[f], &payload_bytes[f], &outs[f], &caps[f], mem, 1);
+    d->frame_errors[f] = status[f] == CLDN_OK ? "" : cldn_b200_last_error();
+    if (status[f] == CLDN_OK && decoded_bytes) decoded_bytes[f] = static_cast<size_t>(points[f] * d->frame_infos[f].point_step);
+  }
+  return result();
 }
 
 extern "C" {
@@ -1452,6 +1741,22 @@ extern "C" {
 int cldn_b200_decode_batch(cldn_decoder_t* d, const cldn_info_t* info, size_t n_frames, const void* const* payloads,
                            const size_t* payload_bytes, void* const* outs, const size_t* out_capacities, int mem, int sync) {
   return guarded([&] { return decode_batch_impl(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, mem, sync); });
+}
+
+int cldn_b200_decode_blobs(cldn_decoder_t* dec, size_t n_frames, const void* const* blobs, const size_t* blob_bytes,
+                           void* const* outs, const size_t* out_capacities, int mem, int32_t* status, size_t* decoded_bytes) {
+  return guarded([&] { return decode_blobs_impl(dec, n_frames, blobs, blob_bytes, outs, out_capacities, mem, status, decoded_bytes); });
+}
+
+const char* cldn_b200_decoder_frame_error(const cldn_decoder_t* dec, size_t f) {
+  return dec && f < dec->frame_errors.size() ? dec->frame_errors[f].c_str() : "";
+}
+
+int cldn_b200_decoder_frame_info(const cldn_decoder_t* dec, size_t f, cldn_info_t* info) {
+  if (!dec || !info) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (f >= dec->frame_infos.size()) { set_error("frame %zu: the last cldn_b200_decode_blobs had %zu frames", f, dec->frame_infos.size()); return CLDN_ERR_INVALID_ARGUMENT; }
+  *info = dec->frame_infos[f];
+  return CLDN_OK;
 }
 
 int cldn_b200_decode(cldn_decoder_t* dec, const cldn_info_t* info, const void* payload, size_t payload_bytes, void* out,

@@ -45,15 +45,15 @@ __global__ void walk_chunks_kernel(const DecLaunch L) {
     uint64_t body = 0;
     uint32_t size = 0;
     if (pos >= F.payload_bytes) {
-      report_error(L.err, DEV_ERR_CHUNK_COUNT);  // "Encoded data ended before all declared points were decoded"
+      report_frame_error(L, f, DEV_ERR_CHUNK_COUNT);  // "Encoded data ended before all declared points were decoded"
     } else if (F.payload_bytes - pos < 4) {
-      report_error(L.err, DEV_ERR_TRUNCATED);    // decode<uint32_t>: not enough input data
+      report_frame_error(L, f, DEV_ERR_TRUNCATED);    // decode<uint32_t>: not enough input data
       pos = F.payload_bytes;
     } else {
       size = load_u32(F.payload + pos);
       pos += 4;
       if (size > F.payload_bytes - pos) {
-        report_error(L.err, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
+        report_frame_error(L, f, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
         size = 0;
         pos = F.payload_bytes;
       }
@@ -63,7 +63,7 @@ __global__ void walk_chunks_kernel(const DecLaunch L) {
     L.chunk_offsets[F.chunk_begin + c] = body;
     L.chunk_sizes[F.chunk_begin + c] = size;
   }
-  if (pos < F.payload_bytes) report_error(L.err, DEV_ERR_CHUNK_COUNT);  // "more chunks than declared points"
+  if (pos < F.payload_bytes) report_frame_error(L, f, DEV_ERR_CHUNK_COUNT);  // "more chunks than declared points"
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -903,7 +903,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const DecLaunch
   // is wrong with a section marks the chunk, and the careful kernels decode it again in the reference's order (regular
   // stream first), so the first error a caller sees is the one the reference would raise.
   const bool side = L.sections_only != 0u && L.side_mode != 0u;
-  uint32_t* const err = side ? &s_side_err : L.err;
+  uint32_t* const err = side ? &s_side_err : frame_err_word(L, s_frame);
   uint32_t pos = 0;
   if (L.sections_only) {
     // the regular stream was decoded by another kernel; sections start where it ended
@@ -911,7 +911,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const DecLaunch
     if (pos > body_bytes) return;  // regular stream failed (error already reported / chunk already marked)
   } else if (plan.values_per_point > 0) {
     const uint32_t used = decode_varint_stream<KT>(body, body_bytes, n_points, static_cast<int>(plan.values_per_point), s_slots,
-                                                   out, plan.point_step, sh, tile_bytes, vals_raw, nanbits, L.err);
+                                                   out, plan.point_step, sh, tile_bytes, vals_raw, nanbits, err);
     if (used == 0xFFFFFFFFu) return;
     pos = used;
   }
@@ -959,7 +959,7 @@ __global__ void __launch_bounds__(kThreads) decode_fixed_kernel(const DecLaunch 
   const uint32_t body_bytes = L.chunk_sizes[gc];
   const uint32_t psize = plan.min_point_bytes;
   if (static_cast<uint64_t>(n_points) * psize > body_bytes) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED);
+    if (threadIdx.x == 0 && blockIdx.x == 0) report_frame_error(L, lo, DEV_ERR_TRUNCATED);
     return;
   }
   uint8_t* out = F.out + static_cast<size_t>(c) * kChunkPoints * plan.point_step;
@@ -999,18 +999,18 @@ __global__ void decode_sequential_kernel(const DecLaunch L) {
   const uint8_t* const body = p;
   if (L.stream_end) L.stream_end[gc] = 0xFFFFFFFFu;  // stays so if the stream turns out to be malformed
   for (uint32_t pt = 0; pt < n_points; ++pt) {
-    if (!plan.uses_v5 && avail < plan.min_point_bytes) { report_error(L.err, DEV_ERR_TRUNCATED); return; }  // v4_codec.cpp:102-104
+    if (!plan.uses_v5 && avail < plan.min_point_bytes) { report_frame_error(L, lo, DEV_ERR_TRUNCATED); return; }  // v4_codec.cpp:102-104
     uint8_t* point = out + static_cast<size_t>(pt) * plan.point_step;
     for (uint32_t k = 0; k < plan.n_ops; ++k) {
       const RegOp& op = plan.ops[k];
       if (op.kind == OP_COPY) {
-        if (avail < op.size) { report_error(L.err, DEV_ERR_TRUNCATED); return; }
+        if (avail < op.size) { report_frame_error(L, lo, DEV_ERR_TRUNCATED); return; }
         if (op.offset[0] != CLDN_SKIP_STORE_OFFSET) store_low_bytes(point + op.offset[0], load_raw_bits(p, op.size), op.size);
         p += op.size; avail -= op.size;
         continue;
       }
       if (op.kind == OP_XOR32 || op.kind == OP_XOR64) {  // field_decoder.hpp:356-370
-        if (avail < op.size) { report_error(L.err, DEV_ERR_TRUNCATED); return; }
+        if (avail < op.size) { report_frame_error(L, lo, DEV_ERR_TRUNCATED); return; }
         const unsigned long long res = load_raw_bits(p, op.size);
         p += op.size; avail -= op.size;
         prev[k] = static_cast<long long>(static_cast<unsigned long long>(prev[k]) ^ res);
@@ -1022,14 +1022,14 @@ __global__ void decode_sequential_kernel(const DecLaunch L) {
         st.prev_bits = static_cast<uint64_t>(prev[k]); st.leading = g_lead[k]; st.trailing = g_trail[k]; st.first = g_first[k] != 0;
         uint64_t v;
         const uint32_t c = gorilla_decode(st, p, avail, &v);
-        if (!c) { report_error(L.err, DEV_ERR_TRUNCATED); return; }
+        if (!c) { report_frame_error(L, lo, DEV_ERR_TRUNCATED); return; }
         p += c; avail -= c;
         prev[k] = static_cast<long long>(st.prev_bits); g_lead[k] = static_cast<uint8_t>(st.leading); g_trail[k] = static_cast<uint8_t>(st.trailing); g_first[k] = 0;
         if (op.offset[0] != CLDN_SKIP_STORE_OFFSET) store_u64(point + op.offset[0], v);
         continue;
       }
       for (int l = 0; l < op.lanes; ++l) {
-        if (avail == 0) { report_error(L.err, DEV_ERR_TRUNCATED); return; }
+        if (avail == 0) { report_frame_error(L, lo, DEV_ERR_TRUNCATED); return; }
         DecSlot s;
         s.offset = op.offset[l]; s.size = op.size; s.mul_f = op.dec_mul_f[l]; s.mul_d = op.dec_mul_d;
         s.kind = op.kind == OP_FLOATN ? SLOT_FLOATN : op.kind == OP_F32_LOSSY ? SLOT_F32 : op.kind == OP_F64_LOSSY ? SLOT_F64 : SLOT_INT;
@@ -1040,7 +1040,7 @@ __global__ void decode_sequential_kernel(const DecLaunch L) {
           continue;
         }
         long long diff;
-        const uint32_t n = read_varint(p, avail, &diff, L.err);
+        const uint32_t n = read_varint(p, avail, &diff, frame_err_word(L, lo));
         if (!n) return;
         p += n; avail -= n;
         long long value;
@@ -1215,7 +1215,7 @@ __global__ void __launch_bounds__(kThreads) decode_mixed_kernel(const DecLaunch 
   uint32_t t0 = 0;     // chunk-body offset of the next point
   while (done < n_points) {
     if (t0 >= size) {  // points are still missing but the bytes are used up: "Truncated encoded data" (v4_codec.cpp:102-104)
-      if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED);
+      if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED);
       return;
     }
     // ---- 1. stage [a0, a0 + kMixTile + kMixLook) with a0 = t0 rounded down to a 16-byte aligned ADDRESS ----
@@ -1330,17 +1330,17 @@ __global__ void __launch_bounds__(kThreads) decode_mixed_kernel(const DecLaunch 
           if (tk.kind == MIX_VAR) {
             long long diff = 0;
             uint8_t nan = 0;
-            if (p >= limit) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+            if (p >= limit) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
             if (bytes[p] == 0 && tk.slot.kind != SLOT_INT) { nan = 1; ++p; }  // NaN marker (field_decoder.cpp:57-61)
             else {
-              const uint32_t n = read_varint(bytes + p, limit - p, &diff, L.err);
+              const uint32_t n = read_varint(bytes + p, limit - p, &diff, frame_err_word(L, s_frame));
               if (!n) { bad = true; break; }
               p += n;
             }
             vals[static_cast<size_t>(threadIdx.x) * n_var + tk.index] = diff;
             nanflag[static_cast<size_t>(threadIdx.x) * n_var + tk.index] = nan;
           } else {
-            if (p + tk.size > limit) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+            if (p + tk.size > limit) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
             raws[static_cast<size_t>(threadIdx.x) * n_fix + tk.index] = load_raw_bits(bytes + p, tk.size);
             p += tk.size;
           }
@@ -1381,12 +1381,12 @@ __global__ void __launch_bounds__(kThreads) decode_mixed_kernel(const DecLaunch 
     __syncthreads();                          // everybody has read the list before the next tile rewrites it
     if (done < n_points) {
       if (end_local == kMixNone || end_local <= mis) {  // the path left the tile through a point this tile cannot delimit
-        if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED);
+        if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED);
         return;
       }
       t0 = static_cast<uint32_t>(a0 + end_local);
     } else {
-      if (end_local == kMixNone) { if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED); return; }
+      if (end_local == kMixNone) { if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); return; }
       if (L.stream_end && threadIdx.x == 0) L.stream_end[gc] = static_cast<uint32_t>(a0 + end_local);  // V5: the sections start here
     }
   }
@@ -1550,7 +1550,7 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
 
   uint32_t done = 0, t0 = 0;
   while (done < n_points) {
-    if (t0 >= size) { if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED); return; }
+    if (t0 >= size) { if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); return; }
     // ---- 1. stage the tile and its terminator bits (as in decode_mixed_kernel) ----
     const uint32_t mis = static_cast<uint32_t>((reinterpret_cast<uintptr_t>(body) + t0) & 15u);
     const int64_t a0 = static_cast<int64_t>(t0) - mis;
@@ -1655,10 +1655,10 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
           if (tk.kind == MIX_VAR) {
             long long diff = 0;
             uint8_t nan = 0;
-            if (p >= limit) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+            if (p >= limit) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
             if (bytes[p] == 0 && tk.slot.kind != SLOT_INT) { nan = 1; ++p; }
             else {
-              const uint32_t n = read_varint(bytes + p, limit - p, &diff, L.err);
+              const uint32_t n = read_varint(bytes + p, limit - p, &diff, frame_err_word(L, s_frame));
               if (!n) { bad = true; break; }
               p += n;
             }
@@ -1669,7 +1669,7 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
             uint32_t len = 8;
             if (!g_first) {
               GorHeader h;
-              if (p >= limit || !gor_header(bytes + p, limit - p, &h)) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+              if (p >= limit || !gor_header(bytes + p, limit - p, &h)) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
               if (h.kind == 0) len = 1;
               else if (h.kind == 1) len = cls[i] ? cls[i] : 9u;  // reuse (before any window: a 65-bit field, like the reference)
               else {
@@ -1677,10 +1677,10 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
                 g_new = (1u << 16) | (h.lead << 8) | ((64u - h.lead - h.meaningful) & 0xFFu);
               }
             }
-            if (p + len > limit) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+            if (p + len > limit) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
             p += len;
           } else {
-            if (p + tk.size > limit) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; break; }
+            if (p + tk.size > limit) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; break; }
             raws[static_cast<size_t>(threadIdx.x) * n_fix + tk.index] = load_raw_bits(bytes + p, tk.size);
             p += tk.size;
           }
@@ -1699,7 +1699,7 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
         st.leading = win ? ((win >> 8) & 0xFFu) : 255u;
         st.trailing = win ? (win & 0xFFu) : 0u;
         uint64_t v = 0;
-        if (!gorilla_decode(st, bytes + g_pos, limit - g_pos, &v)) { report_error(L.err, DEV_ERR_TRUNCATED); bad = true; }
+        if (!gorilla_decode(st, bytes + g_pos, limit - g_pos, &v)) { report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); bad = true; }
         xres = v;  // previous bits 0: the value IS the residual (the first record: the raw bits)
       }
       if (__syncthreads_or(bad ? 1 : 0)) return;
@@ -1742,12 +1742,12 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
     const uint32_t exit_class = s_exit_class;
     __syncthreads();
     if (done < n_points) {
-      if (end_local == kMixNone || end_local <= mis) { if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED); return; }
+      if (end_local == kMixNone || end_local <= mis) { if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); return; }
       t0 = static_cast<uint32_t>(a0 + end_local);
       if (threadIdx.x == 0) s_class = exit_class;
       __syncthreads();
     } else {
-      if (end_local == kMixNone) { if (threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED); return; }
+      if (end_local == kMixNone) { if (threadIdx.x == 0) report_frame_error(L, s_frame, DEV_ERR_TRUNCATED); return; }
       if (L.stream_end && threadIdx.x == 0) L.stream_end[gc] = static_cast<uint32_t>(a0 + end_local);
     }
   }

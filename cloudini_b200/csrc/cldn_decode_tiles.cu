@@ -55,7 +55,7 @@ __global__ void count_tiles_kernel(const DecLaunch L) {
   L.stream_end[gc] = 0xFFFFFFFFu;  // set by the tile that decodes the chunk's last regular value
   const uint32_t chunk = gc - L.frames[lo].chunk_begin;
   const uint32_t n_points = min(kChunkPoints, L.frames[lo].n_points - chunk * kChunkPoints);
-  if (size == 0 && n_points * L.plan->values_per_point > 0) report_error(L.err, DEV_ERR_TRUNCATED);
+  if (size == 0 && n_points * L.plan->values_per_point > 0) report_frame_error(L, lo, DEV_ERR_TRUNCATED);
 }
 
 // single CTA: exclusive scan of chunk_tiles -> chunk_tile_begin[0..n], total in chunk_tile_begin[n]
@@ -697,12 +697,12 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
   if (done >= V) return;
   const uint32_t take = min(tile_cnt, V - done);
   // "ran out of bytes": the chunk's last tile still misses values (v4_codec.cpp:102-104)
-  if (t + 1 == L.chunk_tiles[gc] && done + tile_cnt < V && threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED);
+  if (t + 1 == L.chunk_tiles[gc] && done + tile_cnt < V && threadIdx.x == 0) report_frame_error(L, L.chunk_frame[gc], DEV_ERR_TRUNCATED);
   if (take > 0 && done + take == V && threadIdx.x == (take - 1) / VT) {  // first byte after the regular stream
     L.stream_end[gc] = static_cast<uint32_t>(tile_b0 + run_end_after(tile_bytes, start16[threadIdx.x], (take - 1) - v0) - kTLook);
   }
   const uint32_t n_mine = v0 < take ? min(VT, take - v0) : 0u;  // my values that belong to the regular stream
-  if (badk < n_mine) report_error(L.err, badcode);            // bytes past the stream may be anything: only real values count
+  if (badk < n_mine) report_frame_error(L, L.chunk_frame[gc], badcode);            // bytes past the stream may be anything: only real values count
 
   // ---- per-field segmented sums of my run; the field of value k is (done + v0 + k) % K = (done % K + k) % K ----
   const uint32_t phase = (done + v0) % K;
@@ -756,15 +756,15 @@ __device__ __forceinline__ void walk_frame_publish(const DecLaunch& L, uint32_t 
     uint64_t body = 0;
     uint32_t size = 0;
     if (pos >= F.payload_bytes) {
-      report_error(L.err, DEV_ERR_CHUNK_COUNT);  // "Encoded data ended before all declared points were decoded"
+      report_frame_error(L, f, DEV_ERR_CHUNK_COUNT);  // "Encoded data ended before all declared points were decoded"
     } else if (F.payload_bytes - pos < 4) {
-      report_error(L.err, DEV_ERR_TRUNCATED);    // decode<uint32_t>: not enough input data
+      report_frame_error(L, f, DEV_ERR_TRUNCATED);    // decode<uint32_t>: not enough input data
       pos = F.payload_bytes;
     } else {
       size = load_u32(F.payload + pos);
       pos += 4;
       if (size > F.payload_bytes - pos) {
-        report_error(L.err, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
+        report_frame_error(L, f, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
         size = 0;
         pos = F.payload_bytes;
       }
@@ -777,7 +777,7 @@ __device__ __forceinline__ void walk_frame_publish(const DecLaunch& L, uint32_t 
     st_relaxed_u64(L.chunk_desc + 2ull * gc, tag | (body & 0xFFFFFFFFFFull));
     st_relaxed_u64(L.chunk_desc + 2ull * gc + 1, tag | size);
   }
-  if (pos < F.payload_bytes) report_error(L.err, DEV_ERR_CHUNK_COUNT);  // "more chunks than declared points"
+  if (pos < F.payload_bytes) report_frame_error(L, f, DEV_ERR_CHUNK_COUNT);  // "more chunks than declared points"
 }
 
 // ---- chunk-sequential kernel: a persistent CTA walks the tiles of one chunk after the other (large batches) ---------
@@ -895,7 +895,7 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
       if (!fast_ok) {  // a value longer than 4 bytes or a malformed marker: the careful reader decides
         uint32_t badcode, badk;
         tile_decode_run<VTMAX>(tile_bytes, run_ptr, n_mine, d, nanm, badcode, badk);
-        if (badk < n_mine) report_error(L.err, badcode);
+        if (badk < n_mine) report_frame_error(L, fidx, badcode);
       }
       if (!fast_ok || nanm != 0ull) local = run_reduce_local<K, VTMAX>(d, nanm, n_mine);  // sums with NaN resets
       TRACE(3);
@@ -923,7 +923,7 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
       done += take;
       TRACE(6);
     }
-    if (done < V && threadIdx.x == 0) report_error(L.err, DEV_ERR_TRUNCATED);  // v4_codec.cpp:102-104
+    if (done < V && threadIdx.x == 0) report_frame_error(L, fidx, DEV_ERR_TRUNCATED);  // v4_codec.cpp:102-104
   }
 }
 

@@ -94,7 +94,16 @@ struct DecLaunch {
   uint64_t side_off[kMaxSideFields];
   uint32_t side_mode;          // decode_chunks_kernel, sections_only: 1 = store into the side arrays; any anomaly marks the
                                // chunk (stream_end = 0xFFFFFFFF) for the careful kernels instead of raising the error word
+  uint32_t* frame_err;         // nullptr, or one word per frame (zeroed per launch) that takes that frame's errors
 };
+
+// Error word of frame f: its own word when the launch has per-frame words, else the launch word (so launches without
+// them report exactly as before). A frame's errors go to its own word only: a raised launch word in a launch with
+// per-frame words means an error that no frame claimed.
+template <class Launch>
+__device__ __forceinline__ uint32_t* frame_err_word(const Launch& L, uint32_t f) { return L.frame_err ? L.frame_err + f : L.err; }
+template <class Launch>
+__device__ __forceinline__ void report_frame_error(const Launch& L, uint32_t f, uint32_t code) { atomicCAS(frame_err_word(L, f), 0u, code); }
 
 // The parallel boundary-search decoders, the warp-parallel Gorilla pre-pass and the parallel run-table parse: defaults
 // since round 2 (hardware-green); CLDN_B200_UNMEASURED=0 selects the older one-thread-per-chunk versions (bisecting aid).
@@ -163,6 +172,7 @@ struct Lz4Launch {
   uint32_t* chunk_sizes;       // per global chunk: bytes in its slot
   uint64_t* sizes;             // per frame: bytes written by the pack kernel (0: did not fit)
   uint32_t* err;
+  uint32_t* frame_err;         // decompression: nullptr, or one word per frame (see frame_err_word)
 };
 int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
 int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream);
@@ -183,6 +193,10 @@ struct ZstdLaunch {
 uint32_t zstd_warps_per_cta();
 size_t zstd_lit_scratch_bytes(uint32_t body_cap);
 int launch_zstd_decompress(const ZstdLaunch& Z, cudaStream_t stream);
+
+// ---- headers of device-resident blobs (cldn_lz4.cu) --------------------------------------------------------------------
+// One launch: tab = [n source addresses][n byte counts][n offsets into dst]; blob f's bytes go to dst + offset[f].
+int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaStream_t stream);
 
 uint64_t kernel_launch_count();
 void count_launch(int n = 1);

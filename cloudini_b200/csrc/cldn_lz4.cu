@@ -239,8 +239,8 @@ __global__ void __launch_bounds__(kLzThreads) lz4_decompress_chunks_kernel(const
   if (n != 0xFFFFFFFFu) dsize = lz4_decompress_warp(F.packed_in + body, n, L.scratch + static_cast<size_t>(gc) * L.slot_stride, L.slot_stride);
   if (lane == 0) {
     L.chunk_sizes[gc] = dsize == 0xFFFFFFFFu ? 0u : dsize;
-    if (n == 0xFFFFFFFFu) report_error(L.err, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
-    else if (dsize == 0xFFFFFFFFu) report_error(L.err, DEV_ERR_LZ4);  // "LZ4 decompression failed"
+    if (n == 0xFFFFFFFFu) report_frame_error(L, f, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
+    else if (dsize == 0xFFFFFFFFu) report_frame_error(L, f, DEV_ERR_LZ4);  // "LZ4 decompression failed"
   }
 }
 
@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L,
   if (threadIdx.x == 0) {
     s_pos = pos;
     L.sizes[f] = fits ? pos : 0ull;
-    if (!fits) report_error(L.err, to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : unpack_err);
+    if (!fits) report_error(to_blob ? L.err : frame_err_word(L, f), to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : unpack_err);
   }
   (void)s_pos;
 }
@@ -303,6 +303,20 @@ int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream) {
 int launch_stage2_unpack(const Lz4Launch& L, uint32_t fail_code, cudaStream_t stream) {
   if (L.n_frames == 0) return 0;
   lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, nullptr, 0, 0, fail_code);
+  count_launch(1);
+  return 1;
+}
+
+// One CTA per blob; tab holds n source addresses, n byte counts and n destination offsets.
+__global__ void __launch_bounds__(256) gather_prefixes_kernel(const uint64_t* tab, uint32_t n, uint8_t* dst) {
+  const uint32_t f = blockIdx.x;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(tab[f]);
+  lz_copy(dst + tab[2ull * n + f], src, static_cast<uint32_t>(tab[n + f]), threadIdx.x, blockDim.x);
+}
+
+int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaStream_t stream) {
+  if (n == 0) return 0;
+  gather_prefixes_kernel<<<n, 256, 0, stream>>>(tab, n, dst);
   count_launch(1);
   return 1;
 }

@@ -779,9 +779,9 @@ __global__ void __launch_bounds__(kZsThreads) zstd_decompress_chunks_kernel(cons
     if (n != 0xFFFFFFFFu) dsize = zstd_decompress_warp(&s_zs[warp], F.packed_in + body, n, L.scratch + static_cast<size_t>(gc) * L.slot_stride, Z.body_cap, litbuf);
     if (lane == 0) {
       L.chunk_sizes[gc] = dsize == kZsBad ? 0u : dsize;
-      if (n == 0xFFFFFFFFu) report_error(L.err, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
-      else if (dsize == kZsBad) report_error(L.err, DEV_ERR_ZSTD);    // "ZSTD decompression failed"
-      else if (c + 1u == F.n_chunks && body + n != F.packed_in_bytes) report_error(L.err, DEV_ERR_CHUNK_COUNT);  // more chunks than points
+      if (n == 0xFFFFFFFFu) report_frame_error(L, f, DEV_ERR_CHUNK_SIZE);  // "Invalid chunk size found while decoding"
+      else if (dsize == kZsBad) report_frame_error(L, f, DEV_ERR_ZSTD);    // "ZSTD decompression failed"
+      else if (c + 1u == F.n_chunks && body + n != F.packed_in_bytes) report_frame_error(L, f, DEV_ERR_CHUNK_COUNT);  // more chunks than points
     }
     __syncwarp();
   }

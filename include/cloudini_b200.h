@@ -173,6 +173,27 @@ int cldn_b200_decode(cldn_decoder_t* dec, const cldn_info_t* info, const void* p
 int cldn_b200_decode_batch(cldn_decoder_t* dec, const cldn_info_t* info, size_t n_frames,
                            const void* const* payloads, const size_t* payload_bytes, void* const* outs,
                            const size_t* out_capacities, int mem, int sync);
+/* Complete blobs (header + payload, as PointcloudEncoder::encode writes them), in any mix of layouts, point counts,
+ * wire versions 3..5 and compression options (no reference counterpart: the reference decodes one message per call).
+ * Frames that share a layout and compression option are decoded in ONE fused launch, whatever their point counts
+ * (LZ4 / ZSTD frames: those that also share the points of a chunk, min(points, 32768)). Synchronous for both memory
+ * kinds. With CLDN_MEM_DEVICE the headers are read with one gather launch of every blob's first 4 KB.
+ * status[f] (host array, always filled): CLDN_OK or the status that cldn_b200_decode_header + cldn_b200_decode return
+ * for that blob alone. decoded_bytes[f] (optional): width*height*point_step of the frame, 0 when it failed.
+ * A good frame's output holds exactly what cldn_b200_decode writes (padding bytes untouched); a failed frame's output
+ * bytes are unspecified, and no frame's bytes outside outs[f][0, out_capacities[f]) are written.
+ * Each frame of a fused launch has its own device error word; a frame that failed is decoded once more alone for its
+ * exact status and message, the good frames of its group are not decoded again.
+ * Returns CLDN_OK when every frame decoded. Otherwise it returns the status of the lowest-index failed frame, and
+ * cldn_b200_last_error() reads "frame <f>: <message>". */
+int cldn_b200_decode_blobs(cldn_decoder_t* dec, size_t n_frames, const void* const* blobs, const size_t* blob_bytes,
+                           void* const* outs, const size_t* out_capacities, int mem, int32_t* status,
+                           size_t* decoded_bytes);
+/* Message of frame f of this handle's last cldn_b200_decode_blobs ("" when it decoded). */
+const char* cldn_b200_decoder_frame_error(const cldn_decoder_t* dec, size_t f);
+/* EncodingInfo read from the header of frame f of this handle's last cldn_b200_decode_blobs (zeroed when the header
+ * did not parse). */
+int cldn_b200_decoder_frame_info(const cldn_decoder_t* dec, size_t f, cldn_info_t* info);
 int cldn_b200_decoder_sync(cldn_decoder_t* dec);
 /* Diagnostics of the LAST FloatN batch decode of this handle (no reference counterpart; synchronises the stream):
  * stats[0] = chunks claimed by the chunk-sequential reader, stats[1] = chunks it handed to the careful reader
