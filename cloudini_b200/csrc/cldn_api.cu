@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <mutex>
 #include <new>
 #include <stdexcept>
 #include <utility>
@@ -150,7 +151,9 @@ struct Stage2 {
   size_t (*zstd_compress)(void*, size_t, const void*, size_t, int) = nullptr;
   size_t (*zstd_decompress)(void*, size_t, const void*, size_t) = nullptr;
   unsigned (*zstd_is_error)(size_t) = nullptr;
+  std::mutex mutex;  // handles on several threads may load a library first at the same time
   bool load(int option) {
+    std::lock_guard<std::mutex> lock(mutex);
     if (option == CLDN_COMP_LZ4) {
       if (!lz4) {
         lz4 = dlopen("liblz4.so.1", RTLD_NOW);
@@ -283,6 +286,7 @@ struct cldn_encoder {
   DevBuf<Plan> d_plan;
   DevBuf<uint8_t> d_header;
   DevBuf<uint64_t> d_status;
+  DevBuf<uint32_t> d_ticket;  // tile ticket of the persistent XYZI kernel
   DevBuf<EncFrame> d_frames;
   PinRing<EncFrame> h_frames;
   DevBuf<uint64_t> d_sizes;
@@ -399,7 +403,7 @@ void cldn_b200_encoder_destroy(cldn_encoder_t* e) {
   if (!e) return;
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
-  e->d_plan.release(); e->d_header.release(); e->d_status.release(); e->d_frames.release(); e->h_frames.release();
+  e->d_plan.release(); e->d_header.release(); e->d_status.release(); e->d_ticket.release(); e->d_frames.release(); e->h_frames.release();
   e->d_sizes.release(); e->h_sizes.release(); e->d_err.release(); e->h_err.release(); e->d_in.release(); e->d_out.release();
   e->d_modes.release(); e->d_sec_scratch.release(); e->d_sec_sizes.release(); e->d_sec_excl.release();
   e->d_chunk_frame.release(); e->h_chunk_frame.release(); e->d_hash.release(); e->d_gorilla.release(); e->pipe.release();
@@ -517,6 +521,7 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
     }
   }
   if (int rc = e->d_status.reserve(static_cast<size_t>(tiles) + 1, true)) return rc;
+  if (int rc = e->d_ticket.reserve(1)) return rc;
   e->epoch = (e->epoch + 1) & 0x3FFFFFu;
   if (e->epoch == 0) {  // epoch wrapped: stale words could alias
     CUDA_TRY(cudaMemsetAsync(e->d_status.p, 0, e->d_status.cap * sizeof(uint64_t), e->stream));
@@ -536,6 +541,7 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
   L.tile_points = T;
   L.flags = aligned16 ? kEncInputsAligned16 : 0u;
   L.uniform_tiles = 0;
+  L.tile_ticket = e->d_ticket.p;
   if (n_frames > 0 && hf[0].n_tiles > 0) {
     bool uniform = true;
     for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_tiles == hf[0].n_tiles;

@@ -1789,7 +1789,7 @@ static int launch_sections_only(const DecLaunch& L, cudaStream_t stream, bool si
   S.redo_mode = redo ? 1u : 0u;
   const size_t smem = dec_smem_bytes(false);
   auto k = decode_chunks_kernel<0>;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+  if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
   k<<<L.n_chunks_total, kThreads, smem, stream>>>(S);  // redo: CTAs beyond the redo list return at once
   return 1;
 }
@@ -1850,7 +1850,7 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
       S.sections_only = 1;
       const size_t smem = dec_smem_bytes(false);
       auto k = decode_chunks_kernel<0>;
-      if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+      if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
       k<<<L.n_chunks_total, kThreads, smem, stream>>>(S);
       ++launches;
     }
@@ -1872,7 +1872,7 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
       R.redo_mode = 1;
       const size_t smem = dec_smem_bytes(false);
       auto k = decode_chunks_kernel<0>;
-      if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+      if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
       k<<<L.n_chunks_total, kThreads, smem, stream>>>(R);  // CTAs beyond the redo list return at once; regular stream + sections
       ++launches;
     }
@@ -1905,15 +1905,15 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
       const size_t smem = dec_smem_bytes(f3 || f4);
       if (f4) {
         auto k = decode_chunks_kernel<4>;
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
         k<<<L.n_chunks_total, kThreads, smem, stream>>>(L);
       } else if (f3) {
         auto k = decode_chunks_kernel<3>;
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
         k<<<L.n_chunks_total, kThreads, smem, stream>>>(L);
       } else {
         auto k = decode_chunks_kernel<0>;
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
         k<<<L.n_chunks_total, kThreads, smem, stream>>>(L);
       }
       ++launches;
@@ -1927,14 +1927,14 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
       // V5 sections (if any) are then decoded by the per-chunk section reader from where the stream ended
       if (mixed_plan_ok(plan)) {
         const size_t msmem = mixed_smem_bytes(plan);
-        if (cudaFuncSetAttribute(decode_mixed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(msmem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(decode_mixed_kernel, msmem) != cudaSuccess) return -1;
         DecLaunch M = L;
         const char* mm = getenv("CLDN_B200_MIXED_DECODE");  // "chase": development override (see the kernel)
         M.mix_chase = (mm && mm[0] == 'c') ? 1u : 0u;
         decode_mixed_kernel<<<L.n_chunks_total, kThreads, msmem, stream>>>(M);
       } else if (gorilla_plan_ok(plan)) {
         const size_t gsmem = gorilla_smem_bytes(plan);
-        if (cudaFuncSetAttribute(decode_gorilla_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(gsmem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(decode_gorilla_kernel, gsmem) != cudaSuccess) return -1;
         decode_gorilla_kernel<<<L.n_chunks_total, kThreads, gsmem, stream>>>(L);
       } else {
         decode_sequential_kernel<<<(L.n_chunks_total + 31) / 32, 32, 0, stream>>>(L);
@@ -1945,7 +1945,7 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
         S.sections_only = 1;
         const size_t smem = dec_smem_bytes(false);
         auto k = decode_chunks_kernel<0>;
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+        if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
         k<<<L.n_chunks_total, kThreads, smem, stream>>>(S);
         ++launches;
       }

@@ -909,7 +909,7 @@ template <int K, int FP, bool MIXED, bool ROWS, int NF, bool SIDE>
 static int launch_fast_one(const FastDecParams& Q, const DecLaunch& L, int sm_count, cudaStream_t stream) {
   const size_t smem = decode_fast_smem_bytes(SIDE);
   auto k = decode_floatn_fast_kernel<K, FP, MIXED, ROWS, NF, SIDE>;
-  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+  if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kFT, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
   const uint32_t grid = min(L.n_chunks_total, static_cast<uint32_t>(per_sm * sm_count));

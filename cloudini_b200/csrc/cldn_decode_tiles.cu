@@ -942,7 +942,7 @@ static int launch_floatn_decode(const RegOp& op, const DecLaunch& L, bool sequen
   const uint32_t o3 = K == 4 ? op.offset[3] : 0u;
   if (sequential) {
     auto k = decode_chunks_seq_kernel<K>;
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+    if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kDT, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
     const uint32_t grid = min(L.n_chunks_total, static_cast<uint32_t>(per_sm * sm_count));
@@ -950,20 +950,19 @@ static int launch_floatn_decode(const RegOp& op, const DecLaunch& L, bool sequen
     k<<<grid, kDT, smem, stream>>>(L, op.dec_mul_f[0], op.dec_mul_f[1], op.dec_mul_f[2], m3, op.offset[0], op.offset[1], op.offset[2], o3);
   } else {
     auto k = decode_tiles_kernel<K>;
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+    if (raise_smem_limit(k, smem) != cudaSuccess) return -1;
     k<<<L.tile_grid, kDT, smem, stream>>>(L, op.dec_mul_f[0], op.dec_mul_f[1], op.dec_mul_f[2], m3, op.offset[0], op.offset[1], op.offset[2], o3);
   }
   return 1;
 }
 
 static int device_sm_count() {
-  static int sm_count = 0;
-  if (sm_count == 0) {
-    int dev = 0;
+  static const int sm_count = [] {  // (a function-local static: handles on several threads may ask first at once)
+    int dev = 0, n = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count <= 0) sm_count = 132;  // H100 SXM
-  }
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n > 0 ? n : 132;  // H100 SXM
+  }();
   return sm_count;
 }
 

@@ -14,6 +14,11 @@
 //           the frame's total size.
 #include <stdio.h>
 
+#include <atomic>
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "cldn_device.cuh"
 #include "cldn_kernels.h"
 
@@ -457,23 +462,33 @@ __global__ void __launch_bounds__(kThreads, MINB) encode_floatn_kernel(const Enc
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-static uint64_t g_launches = 0;
-uint64_t kernel_launch_count() { return g_launches; }
-void count_launch(int n) { g_launches += static_cast<uint64_t>(n); }
+static std::atomic<uint64_t> g_launches{0};
+uint64_t kernel_launch_count() { return g_launches.load(std::memory_order_relaxed); }
+void count_launch(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
+
+cudaError_t raise_smem_limit_ptr(const void* kernel, size_t bytes) {
+  static std::mutex mutex;
+  static std::map<std::pair<int, const void*>, size_t> marks;  // highest limit set so far, per device context
+  int dev = 0;
+  if (const cudaError_t e = cudaGetDevice(&dev)) return e;
+  std::lock_guard<std::mutex> lock(mutex);  // check and set together: two raising threads must not leave the smaller value
+  size_t& mark = marks[{dev, kernel}];
+  if (bytes <= mark) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  if (e == cudaSuccess) mark = bytes;
+  return e;
+}
 
 template <typename K>
-static cudaError_t set_smem(K kernel, size_t bytes) {
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
-}
+static cudaError_t set_smem(K* kernel, size_t bytes) { return raise_smem_limit(kernel, bytes); }
 
 // Tuning variant of the FloatN kernel: 0 = I=8 / 2 CTAs per SM (128 regs), 1 = I=8 / 3 CTAs (80 regs),
 // 2 = I=4 / 4 CTAs (64 regs). Chosen once per process (env CLDN_B200_ENC_VARIANT overrides the default).
 static int floatn_variant() {
-  static int v = -1;
-  if (v < 0) {
+  static const int v = [] {
     const char* e = getenv("CLDN_B200_ENC_VARIANT");
-    v = (e && e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 1;
-  }
+    return (e && e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 1;
+  }();
   return v;
 }
 

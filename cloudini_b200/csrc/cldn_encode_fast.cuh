@@ -41,6 +41,8 @@ struct EncFastShared {
   uint32_t wtail[kEW];       // last 4 bytes of every warp's run (top byte = most recent)
   unsigned long long excl;   // look-back result of the group's first tile
   uint32_t scan[kET / 32 + 1];
+  uint32_t first;            // the CTA's first tile and ...
+  uint32_t ticket;           // ... the tile it takes next (thread 0 draws both from L.tile_ticket)
 };
 
 __device__ __forceinline__ float max_nan(float a, float b) {  // NaN if either is NaN (fmaxf would drop it)
@@ -130,16 +132,18 @@ __device__ __noinline__ uint32_t encode_tile_careful(const EncFrame& F, const Fl
 // independent 256-point warp tiles without any CTA barrier (four times as many status words: the look-back gets deeper);
 // warp-private buffers with one barrier per tile, with and without deferring the copy-out by one tile (every warp
 // following the look-back costs more than the two barriers it saves).
-// Persistent CTAs: CTA b takes the tiles b, b + G, b + 2 G, ... of the launch's global tile order (frame-interleaved for
-// uniform batches, so the tiles a look-back depends on are being processed by other CTAs at the same time). While tile i
-// is quantised and packed, tile i + G is already on its way into the other input buffer (cp.async, 16 bytes per lane,
-// straight into the transposed slots): the load latency that a one-tile-per-CTA kernel exposes at every CTA start
-// (measured: a third of all stall samples) is hidden behind the previous tile's arithmetic.
+// Persistent CTAs: every CTA takes its tiles in the launch's global tile order (frame-interleaved for uniform batches, so
+// the tiles a look-back depends on are being processed by other CTAs at the same time) from a ticket counter. While
+// tile i is quantised and packed, the CTA's next tile is already on its way into the other input buffer (cp.async, 16
+// bytes per lane, straight into the transposed slots): the load latency that a one-tile-per-CTA kernel exposes at every
+// CTA start (measured: a third of all stall samples) is hidden behind the previous tile's arithmetic.
 // Also measured (commit 5f46c71 has the code: CLDN_FAST_ENC_PIPE=1/2, removed again): pass 1 of tile i + 1 between pass 2 of tile i and its
 // look-back result, with and without the barrier behind the copy-out: slower either way -- the
 // later inclusive prefix makes every successor's look-back longer than the wait it hides.
-// All G CTAs must be co-resident (the grid is sized by the occupancy query): a CTA spins on aggregates of tiles with a
-// smaller global index, which belong to CTAs that are running.
+// Why tickets: a CTA spins on aggregates of tiles with a smaller global index. A tile is only ever held by a CTA that has
+// started, and a CTA handles its tiles in increasing order, so the smallest unfinished tile is always the current tile
+// of a running CTA and can finish. A fixed assignment (CTA b takes b, b + G, ...) would need all G CTAs resident at
+// once, which no longer holds when kernels of other streams or handles occupy part of the GPU.
 __device__ __forceinline__ void tile_coords(const EncLaunch& L, uint32_t i, uint32_t* fi, uint32_t* t) {
   if (L.uniform_tiles) {
     *fi = i % L.n_frames;
@@ -157,15 +161,22 @@ __global__ void __launch_bounds__(kET, CLDN_FAST_ENC_MINB) encode_xyzi_fast_kern
   __shared__ FloatNParams s_P;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool aligned16 = (L.flags & kEncInputsAligned16) != 0u;
-  const uint32_t G = gridDim.x;
 
   if (blockIdx.x == 0) handle_empty_frames(L);
-  uint32_t i = blockIdx.x;
+  if (threadIdx.x == 0) {
+    sh.first = atomicAdd(L.tile_ticket, 1u);
+    if (sh.first < L.n_tiles_total) {
+      uint32_t f0, t0;
+      tile_coords(L, sh.first, &f0, &t0);
+      s_F[0] = L.frames[f0];
+    }
+    s_P = P;
+  }
+  __syncthreads();
+  const uint32_t i = sh.first;
   if (i >= L.n_tiles_total) return;
   uint32_t fi, t;
   tile_coords(L, i, &fi, &t);
-  if (threadIdx.x == 0) { s_F[0] = L.frames[fi]; s_P = P; }
-  __syncthreads();
 
   // asks for the 1024 points of tile t of frame F into `buf` (transposed slots); false if the tile is not eligible
   auto prefetch = [&](const EncFrame& F, uint32_t tt, uint8_t* buf) -> bool {
@@ -182,13 +193,15 @@ __global__ void __launch_bounds__(kET, CLDN_FAST_ENC_MINB) encode_xyzi_fast_kern
   };
   bool have_cur = prefetch(s_F[0], t, dyn_smem);
   async_commit();
+  if (threadIdx.x == 0) sh.ticket = atomicAdd(L.tile_ticket, 1u);
+  __syncthreads();
 
-  for (uint32_t cur = 0; i < L.n_tiles_total; i += G, cur ^= 1u) {
+  for (uint32_t cur = 0;; cur ^= 1u) {
     const EncFrame& F = s_F[cur];
     uint8_t* buf = dyn_smem + cur * kEBufBytes;            // this tile's transposed input, then its staged output
     uint8_t* stage = buf;
     // ---- the next tile of this CTA goes into the other buffer now ----
-    const uint32_t nxt = i + G;
+    const uint32_t nxt = sh.ticket;   // (rewritten only behind the barriers below)
     bool have_next = false;
     uint32_t nfi = 0, nt = 0;
     if (nxt < L.n_tiles_total) {
@@ -360,7 +373,10 @@ __global__ void __launch_bounds__(kET, CLDN_FAST_ENC_MINB) encode_xyzi_fast_kern
     }
     __syncthreads();  // staged bytes + sh.excl complete (and s_F[cur ^ 1] written)
     finish_tile<kETilePts>(L, F, fi, t, stage, total, sh.excl);
-    __syncthreads();  // this buffer receives the tile after next
+    // the ticket for the tile after next is drawn just before that tile's copies are issued
+    if (threadIdx.x == 0 && nxt < L.n_tiles_total) sh.ticket = atomicAdd(L.tile_ticket, 1u);
+    __syncthreads();  // this buffer receives the tile after next (and sh.ticket is published)
+    if (nxt >= L.n_tiles_total) break;
     have_cur = have_next;
     fi = nfi;
     t = nt;
@@ -395,19 +411,16 @@ static int launch_encode_fast(const Plan& plan, const EncLaunch& L, cudaStream_t
   const size_t smem = kESmemBytes;
   auto k = encode_xyzi_fast_kernel;
   if (set_smem(k, smem) != cudaSuccess) return -1;
-  // persistent grid: every CTA must be resident (they wait for each other's tile sizes)
-  static int resident = 0;
-  if (resident == 0) {
+  // persistent grid of one GPU's worth of CTAs; they take their tiles from the ticket counter, so none has to be resident
+  static const int resident = [&] {
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kET, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    resident = std::max(1, sms) * per_sm;
-#ifdef CLDN_CUSIM
-    resident = static_cast<int>(::cusim::coresident_ctas());  // the emulation runs this many CTAs at a time, not 132 SMs' worth
-#endif
-  }
+    return std::max(1, sms) * per_sm;
+  }();
   const uint32_t grid = std::min<uint32_t>(L.n_tiles_total, static_cast<uint32_t>(resident));
+  if (cudaMemsetAsync(L.tile_ticket, 0, sizeof(uint32_t), stream) != cudaSuccess) return -1;
   k<<<grid, kET, smem, stream>>>(L, P);
   count_launch();
   return 1;

@@ -37,6 +37,7 @@ struct EncLaunch {
   uint32_t tile_points;    // 256 * I (choose_tile_points)
   uint32_t flags;          // kEncInputsAligned16: every frame's input base is 16-byte aligned
   uint32_t uniform_tiles;  // > 0: every frame has exactly this many tiles (frame = tile / uniform_tiles, no search)
+  uint32_t* tile_ticket;   // one word, zeroed per launch: the persistent XYZI kernel's CTAs take their tiles from it in order
 };
 constexpr uint32_t kEncInputsAligned16 = 1u;
 uint32_t choose_tile_points(const Plan& plan);
@@ -199,6 +200,14 @@ int launch_zstd_decompress(const ZstdLaunch& Z, cudaStream_t stream);
 int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaStream_t stream);
 
 uint64_t kernel_launch_count();
-void count_launch(int n = 1);
+void count_launch(int n = 1);  // process-wide, atomic: handles on other threads count into the same total
+
+// Raises `kernel`'s dynamic shared memory limit on the current device to at least `bytes` and never lowers it. The limit
+// is one value per (device, kernel) for the whole process, so a launch site that set exactly what its own launch needs
+// could lower it between another thread's set and that thread's launch, and the other launch would then fail. The limit
+// is a cap, not a reservation: occupancy and the launch itself take the launch's own size.
+cudaError_t raise_smem_limit_ptr(const void* kernel, size_t bytes);
+template <typename K>
+inline cudaError_t raise_smem_limit(K* kernel, size_t bytes) { return raise_smem_limit_ptr((const void*)kernel, bytes); }
 
 }  // namespace cldn

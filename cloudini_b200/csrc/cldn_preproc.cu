@@ -275,7 +275,7 @@ int cldn_b200_viz_lossy_preprocess(cldn_preproc_t* pp, cldn_info_t* info, const 
   PP_CUDA(cudaMemsetAsync(pp->firsts.p, 0xFF, static_cast<size_t>(capacity) * sizeof(uint32_t), pp->stream));
   viz_insert_kernel<<<(n + kThreads - 1) / kThreads, kThreads, 0, pp->stream>>>(L);
   const size_t smem = staged ? static_cast<size_t>(tile_points) * step + 32 : 0;
-  PP_CUDA(cudaFuncSetAttribute(viz_compact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  PP_CUDA(raise_smem_limit(viz_compact_kernel, smem));
   viz_compact_kernel<<<n_tiles, kThreads, smem, pp->stream>>>(L);
   count_launch(2);
   PP_CUDA(cudaGetLastError());

@@ -816,9 +816,9 @@ size_t palette_overflow_scratch_bytes() {
 int launch_encode_sections(const Plan& plan, const SecLaunch& L, cudaStream_t stream) {
   if (L.n_chunks_total == 0) return 0;
   const size_t smem = sizeof(SecShared) + 16;
-  if (cudaFuncSetAttribute(probe_modes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(encode_sections_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(palette_overflow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess) return -1;
+  if (raise_smem_limit(probe_modes_kernel, smem) != cudaSuccess) return -1;
+  if (raise_smem_limit(encode_sections_kernel, smem) != cudaSuccess) return -1;
+  if (raise_smem_limit(palette_overflow_kernel, smem) != cudaSuccess) return -1;
   // fields of <= 4 bytes: the staged writers (values loaded once into shared memory); 64-bit fields: the writers that
   // read the cloud in place. CLDN_B200_SECTIONS_STAGED=0 sends everything to the latter (bisecting aid).
   static const bool staged_on = [] { const char* e = getenv("CLDN_B200_SECTIONS_STAGED"); return !(e && e[0] == '0'); }();
@@ -830,7 +830,7 @@ int launch_encode_sections(const Plan& plan, const SecLaunch& L, cudaStream_t st
   probe_modes_kernel<<<L.n_frames * plan.n_sections, kSecThreads, smem, stream>>>(L2);
   if (staged_on && any_small) {
     const size_t smem2 = sizeof(StagedShared) + 16;
-    if (cudaFuncSetAttribute(encode_sections_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem2)) != cudaSuccess) return -1;
+    if (raise_smem_limit(encode_sections_staged_kernel, smem2) != cudaSuccess) return -1;
     encode_sections_staged_kernel<<<L.n_chunks_total * plan.n_sections, kSecThreads, smem2, stream>>>(L2);
     ++launched;
   }

@@ -275,7 +275,7 @@ enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaEventDefault = 0 };
 
-namespace cusim { int sm_count(); unsigned coresident_ctas(); }
+namespace cusim { int sm_count(); }
 static inline const char* cudaGetErrorString(cudaError_t e) { return e == 0 ? "no error" : "cusim error"; }
 static inline const char* cudaGetErrorName(cudaError_t e) { return e == 0 ? "cudaSuccess" : "cusimError"; }
 static inline cudaError_t cudaGetLastError() { return static_cast<cudaError_t>(::cusim::take_last_error()); }

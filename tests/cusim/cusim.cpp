@@ -131,13 +131,33 @@ struct Cta {
 
 thread_local Cta* g_cta = nullptr;
 thread_local std::vector<std::pair<void*, size_t>> g_shared_regs;  // static __shared__ variables seen on this OS thread
-std::mutex g_pool_mutex;
-std::vector<Cta*> g_pool;  // CTA contexts (fiber stacks) are recycled between launches
+}  // namespace
 
-Cta* acquire_cta() {
+// The emulation's own locks. In the racecheck build they must not order the host threads that launch kernels: a lock
+// that every launch takes would put a happens-before edge between any two host threads' library calls and hide their
+// races. There they are spinlocks on atomics of this (uninstrumented) file, which ThreadSanitizer does not see.
+#if defined(CUSIM_TSAN)
+struct HostLock {
+  std::atomic<bool> held{false};
+  void lock() { while (held.exchange(true, std::memory_order_acquire)) std::this_thread::yield(); }
+  void unlock() { held.store(false, std::memory_order_release); }
+};
+#else
+typedef std::mutex HostLock;
+#endif
+
+namespace {
+
+HostLock g_pool_mutex;
+// CTA contexts (fiber stacks) are recycled between the launches of one host thread (its worker threads are created and
+// joined by it, which orders the reuse; sharing them between host threads would order those threads)
+std::map<std::thread::id, std::vector<Cta*>> g_pool;
+
+Cta* acquire_cta(std::thread::id host) {
   {
-    std::lock_guard<std::mutex> lock(g_pool_mutex);
-    if (!g_pool.empty()) { Cta* c = g_pool.back(); g_pool.pop_back(); g_cta = c; return c; }
+    std::lock_guard<HostLock> lock(g_pool_mutex);
+    std::vector<Cta*>& pool = g_pool[host];
+    if (!pool.empty()) { Cta* c = pool.back(); pool.pop_back(); g_cta = c; return c; }
   }
   Cta* c = new Cta();
   c->stacks = static_cast<char*>(mmap(nullptr, kStackBytes * kMaxThreads, PROT_READ | PROT_WRITE,
@@ -147,10 +167,10 @@ Cta* acquire_cta() {
   g_cta = c;
   return c;
 }
-void release_cta(Cta* c) {
+void release_cta(Cta* c, std::thread::id host) {
   g_cta = nullptr;
-  std::lock_guard<std::mutex> lock(g_pool_mutex);
-  g_pool.push_back(c);
+  std::lock_guard<HostLock> lock(g_pool_mutex);
+  g_pool[host].push_back(c);
 }
 
 void yield_to_scheduler() {
@@ -310,16 +330,6 @@ void run_cta(Cta* c, dim3 grid, dim3 block, uint3 bid) {
 }
 
 }  // namespace
-
-// CTAs the emulation really runs at the same time (one per OS thread): a persistent kernel whose CTAs wait for each other
-// must not launch more than this many (on the GPU the occupancy query gives the corresponding bound)
-unsigned coresident_ctas() {
-  unsigned workers = std::thread::hardware_concurrency();
-  if (const char* e = getenv("CUSIM_WORKERS")) workers = static_cast<unsigned>(atoi(e));
-  if (workers < 1) workers = 1;
-  if (workers > 16) workers = 16;
-  return workers;
-}
 
 int sm_count() {
   const char* e = getenv("CUSIM_SMS");
@@ -535,26 +545,38 @@ void event_forget(void* event) {
   g_events.erase(event);
 }
 
-static std::mutex g_attr_mutex;
+static HostLock g_attr_mutex;
 static std::map<const void*, size_t> g_max_dyn_smem;
-static std::atomic<int> g_last_error{0};
+static thread_local int g_last_error = 0;  // like CUDA's: one error word per host thread
+static HostLock g_launch_mutex;          // the emulated device runs one kernel at a time
 
+// CUSIM_SMEM_MONOTONIC=1: a call that LOWERS a kernel's dynamic shared memory limit fails. The limit is one value per
+// kernel for the whole process, so library code that lowers it can make a launch of another thread, which set a larger
+// limit a moment earlier, fail; code that only ever raises it cannot. This mode finds the lowering calls without threads.
 int set_max_dyn_smem(const void* kernel, int bytes) {
   if (bytes < 0 || bytes > 227 * 1024) return 1;  // cudaErrorInvalidValue
-  std::lock_guard<std::mutex> lock(g_attr_mutex);
+  static const bool monotonic = [] { const char* e = getenv("CUSIM_SMEM_MONOTONIC"); return e && e[0] == '1'; }();
+  std::lock_guard<HostLock> lock(g_attr_mutex);
+  auto it = g_max_dyn_smem.find(kernel);
+  if (monotonic && it != g_max_dyn_smem.end() && static_cast<size_t>(bytes) < it->second) {
+    fprintf(stderr, "cusim: cudaFuncSetAttribute lowers a kernel's dynamic shared memory limit from %zu to %d bytes (CUSIM_SMEM_MONOTONIC)\n", it->second, bytes);
+    return 1;
+  }
   g_max_dyn_smem[kernel] = static_cast<size_t>(bytes);
   return 0;
 }
-int take_last_error() { return g_last_error.exchange(0); }
+int take_last_error() { const int e = g_last_error; g_last_error = 0; return e; }
 
 void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body, const void* kernel) {
   const uint64_t n_ctas = static_cast<uint64_t>(grid.x) * grid.y * grid.z;
   const unsigned n_threads = block.x * block.y * block.z;
+  std::lock_guard<HostLock> one_kernel_at_a_time(g_launch_mutex);
+  const std::thread::id host = std::this_thread::get_id();
   DeviceAccess device_access;
   if (kernel) {
     size_t allowed = 48 * 1024;
     {
-      std::lock_guard<std::mutex> lock(g_attr_mutex);
+      std::lock_guard<HostLock> lock(g_attr_mutex);
       auto it = g_max_dyn_smem.find(kernel);
       if (it != g_max_dyn_smem.end() && it->second > allowed) allowed = it->second;
     }
@@ -579,7 +601,7 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
   if (workers > n_ctas) workers = static_cast<unsigned>(n_ctas);
   std::atomic<uint64_t> next{0};
   auto worker = [&]() {
-    Cta* c = acquire_cta();
+    Cta* c = acquire_cta(host);
     c->body = &body;
 #if CUSIM_ASAN
     // exactly the bytes the launch asked for (rounded to the 16-byte granularity the kernels' staged copies may read),
@@ -612,7 +634,7 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
                       static_cast<unsigned>(i / (static_cast<uint64_t>(grid.x) * grid.y))};
       run_cta(c, grid, block, bid);
     }
-    release_cta(c);
+    release_cta(c, host);
   };
   // always on fresh OS threads: the caller's thread keeps its own (possibly small) stack out of the picture
   std::vector<std::thread> pool;

@@ -5,7 +5,7 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "_shim_roundtrip")
+# The executables are built into the test's temporary directory, never into the source tree (which may be read-only).
 
 
 def _run_env(tmp_path):
@@ -22,38 +22,37 @@ def _run_env(tmp_path):
     return dict(os.environ, LD_LIBRARY_PATH=str(tmp_path / "lib"))
 
 
-def _compile(lib_built):
+def _compile(lib_built, out_dir):
+    exe = os.path.join(str(out_dir), "shim_roundtrip")
     cmd = ["g++", "-std=c++17", "-O1", "-I" + os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "shim_roundtrip.cpp"),
-           "-L" + os.path.dirname(lib_built), "-lcloudini_b200", "-Wl,-rpath," + os.path.dirname(lib_built), "-o", EXE]
+           "-L" + os.path.dirname(lib_built), "-lcloudini_b200", "-Wl,-rpath," + os.path.dirname(lib_built), "-o", exe]
     subprocess.check_call(cmd)
+    return exe
 
 
-def test_shim_compiles_and_links(lib_built):
-    _compile(lib_built)
-    assert os.path.exists(EXE)
+def test_shim_compiles_and_links(lib_built, tmp_path):
+    assert os.path.exists(_compile(lib_built, tmp_path))
 
 
 @pytest.mark.gpu
 def test_shim_roundtrip_on_gpu(lib_built, tmp_path):
-    _compile(lib_built)
-    out = subprocess.run([EXE], capture_output=True, text=True, timeout=120, env=_run_env(tmp_path))
+    exe = _compile(lib_built, tmp_path)
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120, env=_run_env(tmp_path))
     assert out.returncode == 0, out.stdout + out.stderr
     assert "shim_roundtrip: ok" in out.stdout
 
 
 # ---- cloudini_ros shim (include/cloudini_b200/ros_msg_utils.hpp) -------------------------------------------------------
-ROS_EXE = os.path.join(ROOT, "tests", "cpp", "_ros_shim_convert")
-
-
-def _compile_ros(lib_built):
+def _compile_ros(lib_built, out_dir):
+    exe = os.path.join(str(out_dir), "ros_shim_convert")
     cmd = ["g++", "-std=c++17", "-O1", "-I" + os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "ros_shim_convert.cpp"),
-           "-L" + os.path.dirname(lib_built), "-lcloudini_b200", "-Wl,-rpath," + os.path.dirname(lib_built), "-o", ROS_EXE]
+           "-L" + os.path.dirname(lib_built), "-lcloudini_b200", "-Wl,-rpath," + os.path.dirname(lib_built), "-o", exe]
     subprocess.check_call(cmd)
+    return exe
 
 
-def test_ros_shim_compiles_and_links(lib_built):
-    _compile_ros(lib_built)
-    assert os.path.exists(ROS_EXE)
+def test_ros_shim_compiles_and_links(lib_built, tmp_path):
+    assert os.path.exists(_compile_ros(lib_built, tmp_path))
 
 
 # (the GPU run of this executable lives at the end of tests/test_gpu_ros.py: it needs the N3 kernels, which have not

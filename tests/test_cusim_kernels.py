@@ -37,7 +37,7 @@ def _run_gpu_suite(cusim_lib, extra_env, selection):
 
 def test_parity_suite_under_emulation(cusim_lib):
     out = _run_gpu_suite(cusim_lib, {"CLDN_B200_FUZZ": "1", "CLDN_B200_FUZZ_SEEDS": "60"}, ["tests/test_gpu_parity.py", "tests/test_gpu_fast_paths.py", "tests/test_gpu_stage2_device.py", "tests/test_gpu_ros.py",
-                                    "tests/test_gpu_zz_legacy_kernels.py", "tests/test_cpp_shim.py"])
+                                    "tests/test_gpu_zz_legacy_kernels.py", "tests/test_cpp_shim.py", "tests/test_gpu_concurrency.py"])
     assert " passed" in out and "failed" not in out
 
 
@@ -129,6 +129,76 @@ def test_emulation_enforces_the_dynamic_shared_memory_launch_rule(tmp_path):
                            os.path.join(here, "cusim.cpp"), "-o", exe, "-ldl"])
     r = subprocess.run([exe], capture_output=True, text=True, timeout=60)
     assert r.returncode == 0, r.stdout + r.stderr
+    r = subprocess.run([exe], env=dict(os.environ, CUSIM_SMEM_MONOTONIC="1"), capture_output=True, text=True, timeout=60)
+    assert r.returncode == 0, r.stdout + r.stderr
+
+
+def test_dynamic_shared_memory_limits_are_only_ever_raised(cusim_lib):
+    # cudaFuncAttributeMaxDynamicSharedMemorySize is one value per kernel for the whole process. A launch site that set what
+    # its own launch needs could lower it between another thread's set and that thread's launch, which then fails with
+    # cudaErrorInvalidValue. Under CUSIM_SMEM_MONOTONIC=1 every lowering call fails, so a lowering call site is found with
+    # one thread: e.g. viz preprocessing at step 16 and then at step 12 (32,800 -> 24,608 bytes for viz_compact_kernel).
+    out = _run_gpu_suite(cusim_lib, {"CUSIM_SMEM_MONOTONIC": "1"},
+                         ["tests/test_gpu_parity.py", "tests/test_gpu_ros.py", "tests/test_gpu_fast_paths.py", "tests/test_gpu_concurrency.py"])
+    assert " passed" in out and "failed" not in out
+
+
+def test_persistent_encoder_needs_no_co_resident_grid(cusim_lib):
+    # The XYZI encoder launches an occupancy-sized persistent grid (2 SMs x 3 CTAs here) while the emulation runs only 2 CTAs
+    # at a time, and the batch has many more tiles than the grid. A kernel whose CTAs waited for tiles of CTAs that have not
+    # started would stall here until the timeout; the encoder takes its tiles in order from a ticket counter instead.
+    env = dict(os.environ, CLDN_B200_LIB=cusim_lib, CLDN_B200_ALLOW_EMULATION="tests-only", CUSIM_WORKERS="2", CUSIM_SMS="2")
+    code = r"""
+import numpy as np, cloudini_b200 as cb
+from cloudini_b200 import synth
+from oracle.client import best_oracle
+oracle = best_oracle()
+n = 3 * 1024 * 6 + 517                                  # 19 full tiles and a partial one per frame
+info, _ = synth.cloud_c2(n, seed=1)
+clouds = [synth.cloud_c2(n, seed=10 + k)[1] for k in range(4)]
+clouds[1].view(np.float32)[4 * 5000 + 1] = np.nan         # one tile of the exact path
+enc = cb.PointcloudEncoder(info)
+outs = [np.zeros(cb.MaxCompressedSize(info, n, True), dtype=np.uint8) for _ in clouds]
+sizes = enc.encode_batch_host(clouds, outs)
+for c, o, s in zip(clouds, outs, sizes):
+    assert bytes(o[:s]) == oracle.encode(info, c), "differs from the oracle"
+print("encoded", sum(sizes))
+"""
+    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0 and "encoded" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+
+
+def test_concurrent_handles_under_thread_sanitizer(lib_built, tmp_path):
+    # tests/cusim/threads_racecheck_main.cpp: four host threads, each with its own encoder, decoder and preprocessor for its
+    # own layout, through every API; the library's host code is instrumented, so a data race on process-wide state (the
+    # launch counter, lazily initialised statics, the shared memory limits, the stage-2 loader) is a report. Kernel races are
+    # the job of test_racecheck_under_thread_sanitizer: the lenient model here.
+    import platform
+    if platform.machine() != "x86_64":
+        pytest.skip("cusim's context switch is x86-64 only")
+    import build_cusim
+    from cloudini_b200.build import SOURCES
+    try:
+        build_cusim.build_racecheck()   # the instrumented kernels and C ABI (objects next to its own driver)
+    except subprocess.CalledProcessError as e:
+        pytest.skip(f"ThreadSanitizer toolchain unavailable: {e}")
+    here = os.path.join(ROOT, "tests", "cusim")
+    objs = [os.path.join(build_cusim.OUT_DIR, os.path.splitext(s)[0] + "_tsan.o") for s in SOURCES + ["cusim.cpp"]]
+    drv, exe = str(tmp_path / "threads_main.o"), str(tmp_path / "threads_racecheck")
+    subprocess.check_call(["g++", "-std=c++17", "-O0", "-g", "-fPIC", "-pthread", "-w", "-fsanitize=thread", "-I", here, "-I",
+                           os.path.join(ROOT, "include"), "-x", "c++", "-c", os.path.join(here, "threads_racecheck_main.cpp"), "-o", drv])
+    subprocess.check_call(["g++", "-fsanitize=thread", "-pthread", "-o", exe, drv, *objs, "-ldl"])
+    env = dict(os.environ, TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0", CUSIM_WORKERS="2")
+    env.pop("LD_PRELOAD", None)
+    env.pop("CUSIM_TSAN_STRICT", None)
+    r = subprocess.run([exe], env=env, capture_output=True, text=True, timeout=1500)
+    if "FATAL: ThreadSanitizer" in r.stderr:
+        pytest.skip("ThreadSanitizer cannot run in this environment: " + r.stderr[-200:])
+    assert r.returncode == 0 and "threads_racecheck: done" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+    assert "WARNING: ThreadSanitizer" not in r.stderr, r.stderr[-6000:]
+    # the control: a plain counter every job bumps is reported (the emulation's own locks do not order the host threads)
+    r = subprocess.run([exe, "--control-racy"], env=env, capture_output=True, text=True, timeout=1500)
+    assert "WARNING: ThreadSanitizer" in r.stderr and "g_control_counter" in r.stderr, r.stdout[-2000:] + r.stderr[-3000:]
 
 
 def test_host_code_never_dereferences_device_memory(cusim_lib, tmp_path):

@@ -280,15 +280,15 @@ def test_viz_then_encode_matches_reference_pipeline(oracle):
 # ---- the cloudini_ros C++ shim (include/cloudini_b200/ros_msg_utils.hpp) through its converter-step executable ---------
 def test_ros_shim_converter_step_matches_golden(lib_built, golden_ros, tmp_path):
     # the C++ shim reproduces the reference converter's output (golden messages generated from the reference)
-    from test_cpp_shim import ROS_EXE, _compile_ros, _run_env
-    _compile_ros(lib_built)
+    from test_cpp_shim import _compile_ros, _run_env
+    ros_exe = _compile_ros(lib_built, tmp_path)
     for name in ("xyzi_viz", "xyz_organized", "dds_sample_4000"):
         if name not in golden_ros:  # the sample excerpt exists only when the goldens were generated next to the reference tree
             continue
         g = golden_ros[name]
         src, comp, rest = tmp_path / "in.msg", tmp_path / "out.comp", tmp_path / "out.rest"
         src.write_bytes(g["msg"])
-        out = subprocess.run([ROS_EXE, str(src), str(comp), str(rest), repr(g["default_resolution"]), "1" if g["viz"] else "0"],
+        out = subprocess.run([ros_exe, str(src), str(comp), str(rest), repr(g["default_resolution"]), "1" if g["viz"] else "0"],
                              capture_output=True, text=True, timeout=120, env=_run_env(tmp_path))
         assert out.returncode == 0 and "ros_shim_convert: ok" in out.stdout, out.stdout + out.stderr
         assert comp.read_bytes() == g["compressed"], name
