@@ -40,11 +40,15 @@ using namespace cldn;
 
 namespace {
 
-// Grow-only device / pinned-host buffers.
+// Grow-only device / pinned-host buffers, freed with their handle.
 template <typename T>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
   int reserve(size_t n, bool zero = false) {
     if (n <= cap) return CLDN_OK;
     if (p) cudaFree(p);
@@ -61,12 +65,15 @@ struct DevBuf {
     }
     return CLDN_OK;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 template <typename T>
 struct PinBuf {
   T* p = nullptr;
   size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(const PinBuf&) = delete;
+  PinBuf& operator=(const PinBuf&) = delete;
+  ~PinBuf() { if (p) cudaFreeHost(p); }
   int reserve(size_t n) {
     if (n <= cap) return CLDN_OK;
     if (p) cudaFreeHost(p);
@@ -77,7 +84,6 @@ struct PinBuf {
     cap = want;
     return CLDN_OK;
   }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
 
 // Ring of pinned upload slots: a slot is only rewritten by the host after the async copy that read it has completed
@@ -88,6 +94,10 @@ struct PinRing {
   cudaEvent_t ev[SLOTS] = {};
   bool used[SLOTS] = {};
   int next = 0;
+  PinRing() = default;
+  PinRing(const PinRing&) = delete;
+  PinRing& operator=(const PinRing&) = delete;
+  ~PinRing() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
   // returns a host pointer with room for n elements
   int acquire(size_t n, T** out, int* idx) {
     const int i = next;
@@ -104,14 +114,6 @@ struct PinRing {
     used[idx] = true;
     return CLDN_OK;
   }
-  void release() {
-    for (int i = 0; i < SLOTS; ++i) {
-      slot[i].release();
-      if (ev[i]) cudaEventDestroy(ev[i]);
-      ev[i] = nullptr;
-      used[i] = false;
-    }
-  }
 };
 
 // Extra streams + an event pool for the host-pointer path: frame f+1 is uploaded while frame f is encoded and
@@ -119,6 +121,14 @@ struct PinRing {
 struct CopyPipeline {
   cudaStream_t h2d = nullptr, d2h = nullptr;
   std::vector<cudaEvent_t> ev;
+  CopyPipeline() = default;
+  CopyPipeline(const CopyPipeline&) = delete;
+  CopyPipeline& operator=(const CopyPipeline&) = delete;
+  ~CopyPipeline() {
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    if (h2d) cudaStreamDestroy(h2d);
+    if (d2h) cudaStreamDestroy(d2h);
+  }
   int ensure(size_t n_events) {
     if (!h2d) CUDA_TRY(cudaStreamCreateWithFlags(&h2d, cudaStreamNonBlocking));
     if (!d2h) CUDA_TRY(cudaStreamCreateWithFlags(&d2h, cudaStreamNonBlocking));
@@ -128,13 +138,6 @@ struct CopyPipeline {
       ev.push_back(e);
     }
     return CLDN_OK;
-  }
-  void release() {
-    for (cudaEvent_t e : ev) cudaEventDestroy(e);
-    ev.clear();
-    if (h2d) cudaStreamDestroy(h2d);
-    if (d2h) cudaStreamDestroy(d2h);
-    h2d = d2h = nullptr;
   }
 };
 
@@ -403,14 +406,9 @@ void cldn_b200_encoder_destroy(cldn_encoder_t* e) {
   if (!e) return;
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
-  e->d_plan.release(); e->d_header.release(); e->d_status.release(); e->d_ticket.release(); e->d_frames.release(); e->h_frames.release();
-  e->d_sizes.release(); e->h_sizes.release(); e->d_err.release(); e->h_err.release(); e->d_in.release(); e->d_out.release();
-  e->d_modes.release(); e->d_sec_scratch.release(); e->d_sec_sizes.release(); e->d_sec_excl.release();
-  e->d_chunk_frame.release(); e->h_chunk_frame.release(); e->d_hash.release(); e->d_gorilla.release(); e->pipe.release();
-  e->d_s1.release(); e->d_lz_scratch.release(); e->d_lz_chunk_frame.release(); e->d_lz_chunk_sizes.release(); e->d_lz_frames.release();
-  e->h_lz_frames.release(); e->h_lz_chunk_frame.release();
-  if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
-  delete e;
+  const cudaStream_t own = e->own_stream ? e->stream : nullptr;
+  delete e;  // the buffers free themselves
+  if (own) cudaStreamDestroy(own);
 }
 
 int cldn_b200_encoder_header(const cldn_encoder_t* enc, const uint8_t** header, size_t* header_bytes) {
@@ -625,24 +623,58 @@ static int guarded(Fn&& fn) {
   }
 }
 
+// The reference's checks of one frame to encode, in its order (cloudini.cpp:523-534). `full` is the layout with the
+// compression the blob declares and `hdr` the header bytes written in front; *need is the worst-case blob size.
+static int check_encode_frame(const cldn_info_t& full, size_t hdr, size_t cloud_bytes, size_t out_capacity, size_t* need) {
+  if (full.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (cloud_bytes % full.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
+  bool ok;
+  *need = max_compressed_size(full, cloud_bytes / full.point_step, false, &ok) + hdr;
+  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
+  if (out_capacity < *need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+  return CLDN_OK;
+}
+
+// Device-pointer batches: the blob sizes into written_host, if asked for (one read-back, synchronises).
+static int read_written(cldn_encoder* e, size_t n_frames, size_t* written_host) {
+  if (!written_host) return CLDN_OK;
+  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+  for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
+  return CLDN_OK;
+}
+
+// Host-pointer staging: n byte ranges at 256-byte-aligned offsets of `buf`, which grows to hold them with 256 bytes to
+// spare; at[f] is where range f starts.
+static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std::vector<void*>& at) {
+  std::vector<size_t> off(n);
+  size_t total = 0;
+  for (size_t f = 0; f < n; ++f) {
+    off[f] = total;
+    total += (bytes[f] + 255) & ~size_t(255);
+  }
+  if (int rc = buf.reserve(total + 256)) return rc;
+  at.resize(n);
+  for (size_t f = 0; f < n; ++f) at[f] = buf.p + off[f];
+  return CLDN_OK;
+}
+
 // Device pointers in, device pointers out, compression LZ4: stage 1 into an internal arena, one LZ4 block per chunk on the
 // device (cldn_lz4.cu), blobs packed behind their headers. Nothing crosses PCIe except the 8-byte sizes, if asked for.
 static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                                    void* const* outs, const size_t* out_capacities, int write_header) {
   const cldn_info_t& info = e->info;  // compression NONE: what the stage-1 kernels produce
-  if (info.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
   cldn_info_t full = info;
   full.compression_opt = CLDN_COMP_LZ4;
   const size_t hdr = write_header ? e->header.size() : 0;
   std::vector<size_t> s1_off(n_frames), s1_cap(n_frames);
   size_t arena = 0, chunks = 0, max_chunk = 0;
   for (size_t f = 0; f < n_frames; ++f) {
-    if (cloud_bytes[f] % info.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
+    size_t need;
+    if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
     const size_t n = cloud_bytes[f] / info.point_step;
     bool ok;
-    const size_t need = max_compressed_size(full, n, false, &ok) + hdr;  // cloudini.cpp:530-534
-    if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-    if (out_capacities[f] < need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
     s1_cap[f] = max_compressed_size(info, n, false, &ok) + 64 * ((n + kChunkPoints - 1) / kChunkPoints + 1);
     s1_off[f] = arena;
     arena += (s1_cap[f] + 255) & ~size_t(255);
@@ -684,7 +716,7 @@ static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void*
   if (int rc = e->h_lz_frames.commit(hf_slot, e->stream)) return rc;
   if (chunks) CUDA_TRY(cudaMemcpyAsync(e->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
   if (int rc = e->h_lz_chunk_frame.commit(hcf_slot, e->stream)) return rc;
-  Lz4Launch Z;
+  Lz4Launch Z{};
   Z.frames = e->d_lz_frames.p;
   Z.n_frames = static_cast<uint32_t>(n_frames);
   Z.n_chunks_total = static_cast<uint32_t>(chunks);
@@ -694,7 +726,6 @@ static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void*
   Z.chunk_sizes = e->d_lz_chunk_sizes.p;
   Z.sizes = e->d_sizes.p;   // the pack kernel overwrites the stage-1 sizes with the blob sizes (it runs after every reader)
   Z.err = e->d_err.p;
-  Z.frame_err = nullptr;
   if (launch_lz4_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) { set_error("LZ4 kernel launch failed"); return CLDN_ERR_CUDA; }
   CUDA_TRY(cudaGetLastError());
   return CLDN_OK;
@@ -709,35 +740,29 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   }
   if (n_frames == 0) return CLDN_OK;
   CUDA_TRY(cudaSetDevice(e->device));
-  if (mem == CLDN_MEM_DEVICE && e->stage2 == CLDN_COMP_LZ4) {
-    if (int rc = encode_batch_device_lz4(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
-    if (written_host) {
-      if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-      CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-      if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-      for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
+  if (mem == CLDN_MEM_DEVICE) {
+    if (e->stage2 != CLDN_COMP_NONE && e->stage2 != CLDN_COMP_LZ4) {
+      set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
+      return CLDN_ERR_UNSUPPORTED;
     }
-    return CLDN_OK;
+    const int rc = e->stage2 == CLDN_COMP_LZ4
+                       ? encode_batch_device_lz4(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)
+                       : encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header);
+    if (rc) return rc;
+    return read_written(e, n_frames, written_host);
   }
-  if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE) {
-    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
-    return CLDN_ERR_UNSUPPORTED;
-  }
-  if (mem == CLDN_MEM_HOST && e->stage2 != CLDN_COMP_NONE) {
+  if (mem != CLDN_MEM_HOST) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  const size_t hdr = write_header ? e->header.size() : 0;
+  if (e->stage2 != CLDN_COMP_NONE) {
     if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
     // stage 1 on the GPU, then every chunk through the system compressor (not pipelined: this is not the product path)
     cldn_info_t full = e->info;
     full.compression_opt = static_cast<uint8_t>(e->stage2);
-    const size_t hdr = write_header ? e->header.size() : 0;
     for (size_t f = 0; f < n_frames; ++f) {
-      if (e->info.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
-      if (cloud_bytes[f] % e->info.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
-      const size_t n = cloud_bytes[f] / e->info.point_step;
+      size_t need;
+      if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
       bool ok;
-      const size_t need = max_compressed_size(full, n, false, &ok) + hdr;  // cloudini.cpp:530-534
-      if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-      if (out_capacities[f] < need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-      size_t cap1 = max_compressed_size(e->info, n, false, &ok);
+      size_t cap1 = max_compressed_size(e->info, cloud_bytes[f] / e->info.point_step, false, &ok);
       if (int rc = e->d_in.reserve(cloud_bytes[f] + 256)) return rc;
       if (int rc = e->d_out.reserve(cap1 + 256)) return rc;
       if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(e->d_in.p, clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
@@ -759,31 +784,11 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     }
     return CLDN_OK;
   }
-  if (mem == CLDN_MEM_DEVICE) {
-    if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
-    if (written_host) {
-      if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-      CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-      if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-      for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
-    }
-    return CLDN_OK;
-  }
-  if (mem != CLDN_MEM_HOST) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
   // ---- host path: H2D -> kernels -> D2H (sizes first, then exactly the encoded bytes) ----
-  size_t in_total = 0, out_total = 0;
-  std::vector<size_t> in_off(n_frames), out_off(n_frames), caps(n_frames);
-  const size_t hdr = write_header ? e->header.size() : 0;
+  std::vector<size_t> caps(n_frames);
   for (size_t f = 0; f < n_frames; ++f) {
-    if (e->info.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
-    if (cloud_bytes[f] % e->info.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
-    bool ok;
-    const size_t need = max_compressed_size(e->info, cloud_bytes[f] / e->info.point_step, false, &ok) + hdr;
-    if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-    if (out_capacities[f] < need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-    in_off[f] = in_total;
-    in_total += (cloud_bytes[f] + 255) & ~size_t(255);
-    out_off[f] = out_total;
+    size_t need;
+    if (int rc = check_encode_frame(e->info, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
     // A committed V5 mode can exceed the reference's own worst-case formula (DeltaRle on a 64-bit field: 11 bytes per
     // value against the 10 it budgets); the reference then succeeds iff the caller's buffer is large enough. Stage with
     // room for the real worst case, never more than the caller gave: the kernels check every store against this bound.
@@ -792,20 +797,18 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
       if (e->plan.sections[s2].bpv == 8) worst += cloud_bytes[f] / e->info.point_step + 16 * ((cloud_bytes[f] / e->info.point_step) / kChunkPoints + 1);
     }
     caps[f] = std::min(out_capacities[f], worst);
-    out_total += (caps[f] + 255) & ~size_t(255);
   }
-  if (int rc = e->d_in.reserve(in_total + 256)) return rc;
-  if (int rc = e->d_out.reserve(out_total + 256)) return rc;
+  std::vector<void*> din, dout;
+  if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, din)) return rc;
+  if (int rc = stage_layout(e->d_out, n_frames, caps.data(), dout)) return rc;
   if (int rc = e->pipe.ensure(2 * n_frames)) return rc;
   if (int rc = e->h_sizes.reserve(n_frames)) return rc;
   // frame f: upload on the h2d stream -> encode on the handle's stream -> 8-byte size read-back
   for (size_t f = 0; f < n_frames; ++f) {
-    const void* din = e->d_in.p + in_off[f];
-    void* dout = e->d_out.p + out_off[f];
-    if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(e->d_in.p + in_off[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
+    if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(din[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
     CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f], e->pipe.h2d));
     CUDA_TRY(cudaStreamWaitEvent(e->stream, e->pipe.ev[2 * f], 0));
-    if (int rc = encode_batch_device(e, 1, &din, &cloud_bytes[f], &dout, &caps[f], write_header)) return rc;
+    if (int rc = encode_batch_device(e, 1, &din[f], &cloud_bytes[f], &dout[f], &caps[f], write_header)) return rc;
     CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p + f, e->d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
     CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f + 1], e->stream));
   }
@@ -818,7 +821,7 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
       set_error("Output buffer too small for uncompressed chunk");
       return CLDN_ERR_BUFFER_TOO_SMALL;
     }
-    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], e->d_out.p + out_off[f], sz, cudaMemcpyDeviceToHost, e->pipe.d2h));
+    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], sz, cudaMemcpyDeviceToHost, e->pipe.d2h));
     if (written_host) written_host[f] = sz;
   }
   CUDA_TRY(cudaStreamSynchronize(e->pipe.d2h));
@@ -948,7 +951,7 @@ static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
 // `frame_points` (optional): points of every frame; nullptr gives every frame info.width * info.height points.
 static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
                                const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
-                               const uint64_t* frame_points = nullptr) {
+                               const uint64_t* frame_points) {
   d->sections_ahead = false;
   if (int rc = decoder_update_plan(d, info)) return rc;
   const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
@@ -982,8 +985,7 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
   if (int rc = d->d_chunk_sizes.reserve(static_cast<size_t>(chunks) + 1)) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->d_frames.p, hf, n_frames * sizeof(DecFrame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_frames.commit(hf_slot, d->stream)) return rc;
-  DecLaunch L;
-  L.mix_chase = 0;
+  DecLaunch L{};
   L.par_runs = unmeasured_kernels_enabled() ? 1u : 0u;
   L.frames = d->d_frames.p;
   L.n_frames = static_cast<uint32_t>(n_frames);
@@ -992,43 +994,23 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
   L.chunk_offsets = d->d_chunk_offsets.p;
   L.chunk_sizes = d->d_chunk_sizes.p;
   L.err = d->d_err.p;
-  L.chunk_frame = nullptr; L.tile_chunk = nullptr;
-  L.chunk_tiles = nullptr; L.chunk_tile_begin = nullptr; L.stream_end = nullptr; L.tstatus = nullptr; L.tsums = nullptr;
-  L.tile_capacity = 0; L.tile_grid = 0; L.epoch = 0; L.trace = nullptr; L.chunk_counter = nullptr; L.sections_only = 0;
-  L.chunk_desc = nullptr; L.desc_tag = 0; L.uniform_chunks = 0; L.redo_list = nullptr; L.redo_mode = 0;
-  L.side = nullptr; L.side_mode = 0;
   L.frame_err = d->frame_err;
-  for (int s = 0; s < kMaxSideFields; ++s) L.side_off[s] = 0;
   if (d->plan.n_sections > 0 && chunks > 0 && (d->plan.regular_overlap || !(d->plan.all_varint || d->plan.n_ops == 0))) {
     // V5 with raw / XOR / Gorilla fields in the regular stream: the per-chunk parser records where the sections start
     if (int rc = d->d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
     L.stream_end = d->d_stream_end.p;
   }
-  const char* force_chunk = getenv("CLDN_B200_FORCE_CHUNK_DECODE");
+  const char* force_env = getenv("CLDN_B200_FORCE_CHUNK_DECODE");
+  const bool force_chunk = force_env && force_env[0] == '1';
   const bool fast_general = !d->plan.floatn_only && chunks > 0 && decode_fast_general_plan(d->plan) &&
-                            decode_tiles_sequential(static_cast<uint32_t>(chunks)) && decode_fast_enabled() && !(force_chunk && force_chunk[0] == '1');
+                            decode_tiles_sequential(static_cast<uint32_t>(chunks)) && decode_fast_enabled() && !force_chunk;
+  const bool tile_parallel = d->plan.floatn_only && chunks > 0 && !force_chunk;
   if (fast_general) {
     // float-varint streams with scalar lossy fields (Velodyne XYZIRT ...): fast chunk-sequential reader + redo list
     if (int rc = d->d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    if (int rc = d->d_counter.reserve(4, true)) return rc;
-    if (int rc = d->d_redo.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    const size_t had = d->d_chunk_desc.cap;
-    if (int rc = d->d_chunk_desc.reserve(2 * static_cast<size_t>(chunks) + 2)) return rc;
-    d->desc_tag = (d->desc_tag + 1) & 0xFFFFFFu;
-    if (d->d_chunk_desc.cap != had || d->desc_tag == 0) {
-      CUDA_TRY(cudaMemsetAsync(d->d_chunk_desc.p, 0, d->d_chunk_desc.cap * sizeof(uint64_t), d->stream));
-      if (d->desc_tag == 0) d->desc_tag = 1;
-    }
     L.stream_end = d->d_stream_end.p;
-    L.chunk_counter = d->d_counter.p;
-    L.redo_list = d->d_redo.p;
-    L.chunk_desc = d->d_chunk_desc.p;
-    L.desc_tag = d->desc_tag;
-    bool uniform = n_frames > 0 && hf[0].n_chunks > 0;
-    for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
-    L.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
   }
-  if (d->plan.floatn_only && chunks > 0 && !(force_chunk && force_chunk[0] == '1')) {
+  if (tile_parallel) {
     // tile-parallel path: host upper bound on the tile count (every chunk adds at most 2 tiles of rounding/misalignment)
     uint64_t tiles = 0;
     for (size_t f = 0; f < n_frames; ++f) tiles += payload_bytes[f] / decode_tile_bytes() + 2ull * hf[f].n_chunks + 1;
@@ -1059,39 +1041,38 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
     L.tile_capacity = static_cast<uint32_t>(d->d_tstatus.cap);
     L.tile_grid = static_cast<uint32_t>(tiles);
     L.epoch = d->epoch;
+  }
+  if (fast_general || tile_parallel) {
+    // chunk claim counters, the careful kernel's redo list and the self-validating chunk descriptors
     if (int rc = d->d_counter.reserve(4, true)) return rc;
-    L.chunk_counter = d->d_counter.p;
     if (int rc = d->d_redo.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    const size_t had = d->d_chunk_desc.cap;
+    if (int rc = d->d_chunk_desc.reserve(2 * static_cast<size_t>(chunks) + 2)) return rc;
+    d->desc_tag = (d->desc_tag + 1) & 0xFFFFFFu;
+    if (d->d_chunk_desc.cap != had || d->desc_tag == 0) {  // fresh memory or tag wrap: no stale word may carry a live tag
+      CUDA_TRY(cudaMemsetAsync(d->d_chunk_desc.p, 0, d->d_chunk_desc.cap * sizeof(uint64_t), d->stream));
+      if (d->desc_tag == 0) d->desc_tag = 1;
+    }
+    L.chunk_counter = d->d_counter.p;
     L.redo_list = d->d_redo.p;
-    {
-      const size_t had = d->d_chunk_desc.cap;
-      if (int rc = d->d_chunk_desc.reserve(2 * static_cast<size_t>(chunks) + 2)) return rc;
-      d->desc_tag = (d->desc_tag + 1) & 0xFFFFFFu;
-      if (d->d_chunk_desc.cap != had || d->desc_tag == 0) {  // fresh memory or tag wrap: no stale word may carry a live tag
-        CUDA_TRY(cudaMemsetAsync(d->d_chunk_desc.p, 0, d->d_chunk_desc.cap * sizeof(uint64_t), d->stream));
-        if (d->desc_tag == 0) d->desc_tag = 1;
-      }
-      L.chunk_desc = d->d_chunk_desc.p;
-      L.desc_tag = d->desc_tag;
-      bool uniform = n_frames > 0 && hf[0].n_chunks > 0;
-      for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
-      L.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
-    }
-    if (getenv("CLDN_B200_TRACE")) {
-      if (int rc = d->d_trace.reserve(std::max<size_t>(static_cast<size_t>(tiles), static_cast<size_t>(chunks) * 80) * 8 + 8, true)) return rc;
-      L.trace = d->d_trace.p;
-    }
+    L.chunk_desc = d->d_chunk_desc.p;
+    L.desc_tag = d->desc_tag;
+    bool uniform = n_frames > 0 && hf[0].n_chunks > 0;
+    for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
+    L.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
+  }
+  if (tile_parallel && getenv("CLDN_B200_TRACE")) {
+    if (int rc = d->d_trace.reserve(std::max<size_t>(L.tile_grid, static_cast<size_t>(chunks) * 80) * 8 + 8, true)) return rc;
+    L.trace = d->d_trace.p;
   }
   d->fast_launched = L.redo_list != nullptr && decode_tiles_sequential(L.n_chunks_total) && decode_fast_enabled() && !d->plan.regular_overlap;
-  if (d->fast_launched && L.chunk_desc && L.stream_end && L.chunk_counter && decode_side_plan(d->plan) && decode_fast_general_plan(d->plan) &&
-      !(force_chunk && force_chunk[0] == '1')) {
+  if (d->fast_launched && L.chunk_desc && L.stream_end && L.chunk_counter && decode_side_plan(d->plan) && decode_fast_general_plan(d->plan) && !force_chunk) {
     // V5 sections ahead of the regular stream: compact per-chunk arrays the fast reader merges into the rows (DecLaunch::side)
     const size_t side_bytes = decode_side_bytes(d->plan, chunks, L.side_off);
     if (int rc = d->d_side.reserve(side_bytes + 256)) return rc;
     L.side = d->d_side.p;
   }
   d->sections_ahead = decode_side_active(d->plan, L);
-  (void)fast_general;
   d->fast_chunks = d->fast_launched ? L.n_chunks_total : 0u;
   if (launch_decode(d->plan, L, d->stream) < 0) { set_error("decode kernel launch failed"); return CLDN_ERR_CUDA; }
   CUDA_TRY(cudaGetLastError());
@@ -1127,15 +1108,9 @@ void cldn_b200_decoder_destroy(cldn_decoder_t* d) {
   if (!d) return;
   cudaSetDevice(d->device);
   if (d->stream) cudaStreamSynchronize(d->stream);
-  d->d_plan.release(); d->d_frames.release(); d->h_frames.release(); d->d_chunk_offsets.release(); d->d_chunk_sizes.release();
-  d->d_err.release(); d->h_err.release(); d->d_in.release(); d->d_out.release();
-  d->d_chunk_tiles.release(); d->d_chunk_tile_begin.release(); d->d_stream_end.release(); d->d_tsums.release(); d->d_tstatus.release(); d->d_chunk_frame.release(); d->d_tile_chunk.release(); d->d_trace.release(); d->d_counter.release(); d->d_redo.release(); d->d_side.release(); d->d_chunk_desc.release(); d->pipe.release();
-  d->d_s1.release(); d->d_lz_scratch.release(); d->d_lz_chunk_frame.release(); d->d_lz_chunk_sizes.release(); d->d_lz_frames.release();
-  d->d_lz_sizes.release(); d->h_lz_sizes.release(); d->h_lz_frames.release(); d->h_lz_chunk_frame.release(); d->d_zs_lit.release();
-  d->d_blob_tab.release(); d->h_blob_tab.release(); d->d_prefix.release(); d->h_prefix.release();
-  d->d_frame_err.release(); d->h_frame_err.release();
-  if (d->own_stream && d->stream) cudaStreamDestroy(d->stream);
-  delete d;
+  const cudaStream_t own = d->own_stream ? d->stream : nullptr;
+  delete d;  // the buffers free themselves
+  if (own) cudaStreamDestroy(own);
 }
 
 int cldn_b200_decoder_sync(cldn_decoder_t* d) {
@@ -1201,80 +1176,6 @@ struct FrameChunks {
   }
 };
 
-// Frame and chunk tables of a stage-2 decompression launch (arena `s1`, laid out by FrameChunks::place).
-static void fill_stage2_frames(uint8_t* s1, const FrameChunks& fc, size_t n_frames, const void* const* payloads,
-                               const size_t* payload_bytes, Lz4Frame* hf, uint32_t* hcf) {
-  uint32_t cb = 0;
-  for (size_t f = 0; f < n_frames; ++f) {
-    Lz4Frame& F = hf[f];
-    memset(&F, 0, sizeof(F));
-    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
-    F.packed_in_bytes = payload_bytes[f];
-    F.plain_out = s1 + fc.s1_off[f];
-    F.plain_cap = fc.s1_cap[f];
-    F.n_chunks = static_cast<uint32_t>(fc.frame_chunks(f));
-    F.chunk_begin = cb;
-    for (uint32_t c = 0; c < F.n_chunks; ++c) hcf[cb + c] = static_cast<uint32_t>(f);
-    cb += F.n_chunks;
-  }
-}
-
-// Device pointers, compression LZ4: every chunk's block is decompressed on the device into a slot, the slots are re-framed
-// into a stage-1 payload per frame (internal arena) and the ordinary stage-1 decode runs on that. One read-back of the
-// frames' stage-1 sizes (8 bytes each) sits between the two.
-static int decode_batch_device_lz4(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                   const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
-                                   const uint64_t* frame_points = nullptr) {
-  cldn_info_t plain = info;
-  plain.compression_opt = CLDN_COMP_NONE;
-  FrameChunks fc;
-  if (int rc = fc.init(info, n_frames, frame_points)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) {
-    if (out_capacities[f] < fc.points[f] * info.point_step) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-  }
-  bool ok;
-  const size_t max_chunk = max_compressed_size(plain, std::min<size_t>(fc.max_points, kChunkPoints), false, &ok) + 64;
-  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-  const size_t slot = (max_chunk + 15) & ~size_t(15);
-  fc.place(slot);
-  const size_t chunks = fc.chunks;
-  if (chunks > 0x7FFFFFFFull || slot > 0xFFFFFFF0ull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = d->d_s1.reserve(std::max<size_t>(fc.arena, 256))) return rc;
-  if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
-  if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
-  if (int rc = d->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
-  if (int rc = d->d_lz_frames.reserve(n_frames)) return rc;
-  if (int rc = d->d_lz_sizes.reserve(n_frames)) return rc;
-  if (int rc = d->h_lz_sizes.reserve(n_frames)) return rc;
-  Lz4Frame* hf = nullptr; int hf_slot = 0;
-  uint32_t* hcf = nullptr; int hcf_slot = 0;
-  if (int rc = d->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
-  if (int rc = d->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
-  fill_stage2_frames(d->d_s1.p, fc, n_frames, payloads, payload_bytes, hf, hcf);
-  CUDA_TRY(cudaMemcpyAsync(d->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, d->stream));
-  if (int rc = d->h_lz_frames.commit(hf_slot, d->stream)) return rc;
-  if (chunks) CUDA_TRY(cudaMemcpyAsync(d->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
-  if (int rc = d->h_lz_chunk_frame.commit(hcf_slot, d->stream)) return rc;
-  Lz4Launch Z;
-  Z.frames = d->d_lz_frames.p;
-  Z.n_frames = static_cast<uint32_t>(n_frames);
-  Z.n_chunks_total = static_cast<uint32_t>(chunks);
-  Z.chunk_frame = d->d_lz_chunk_frame.p;
-  Z.scratch = d->d_lz_scratch.p;
-  Z.slot_stride = static_cast<uint32_t>(slot);
-  Z.chunk_sizes = d->d_lz_chunk_sizes.p;
-  Z.sizes = d->d_lz_sizes.p;
-  Z.err = d->d_err.p;
-  Z.frame_err = d->frame_err;
-  if (launch_lz4_decompress(Z, d->stream) < 0) { set_error("LZ4 kernel launch failed"); return CLDN_ERR_CUDA; }
-  CUDA_TRY(cudaMemcpyAsync(d->h_lz_sizes.p, d->d_lz_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, d->stream));
-  if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged blocks stop here
-  std::vector<const void*> p1(n_frames);
-  std::vector<size_t> b1(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) { p1[f] = d->d_s1.p + fc.s1_off[f]; b1[f] = static_cast<size_t>(d->h_lz_sizes.p[f]); }
-  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities, frame_points);
-}
-
 // Bound of one decompressed chunk, as the host-pointer API has always passed it to ZSTD_decompress / LZ4_decompress_safe:
 // the stage-1 worst case of a chunk, or the whole frame's bytes if larger (DecompressChunk's bound is w*h*step,
 // cloudini.cpp:672-675), plus 64.
@@ -1292,36 +1193,49 @@ static bool zstd_host_route() {
   return v && v[0] == '1';
 }
 
-// Device pointers, compression ZSTD: the LZ4 path's structure (slots, chunk table, re-framing) with the ZSTD decompressor
-// of cldn_zstd.cu. A chunk may decompress to max_body bytes (the host-pointer bound) but not beyond its slot, which holds
-// the stage-1 worst case of a 32768-point chunk: a larger chunk body cannot be a stage-1 chunk and is refused as damaged.
-// On return p1 / b1 are the frames' stage-1 payloads in the internal arena (one read-back of their sizes).
+// Stage 2 on the device, LZ4 or ZSTD (info.compression_opt): every chunk is decompressed into a slot (cldn_lz4.cu,
+// cldn_zstd.cu) and the slots are re-framed into one stage-1 payload per frame in the decoder's arena. On return p1 / b1
+// are those payloads, behind one read-back of their sizes (8 bytes per frame) and one synchronisation. A slot holds the
+// stage-1 worst case of a 32768-point chunk: a larger chunk body cannot be a stage-1 chunk and is refused as damaged.
 // `frame_points` as decode_batch_device takes it: the frames of one launch share one chunk bound (that of the largest).
-static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads, const size_t* payload_bytes,
-                              std::vector<const void*>& p1, std::vector<size_t>& b1, const uint64_t* frame_points = nullptr) {
+// `out_capacities`, if given, are checked before any scratch is sized from the (untrusted) header.
+static int stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
+                         const size_t* payload_bytes, const size_t* out_capacities, const uint64_t* frame_points,
+                         std::vector<const void*>& p1, std::vector<size_t>& b1) {
+  const bool zstd = info.compression_opt == CLDN_COMP_ZSTD;
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
+  // ZSTD checks the capacity before the point counts, LZ4 after them; the two forms differ for point_step 0
+  const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
+  for (size_t f = 0; zstd && out_capacities && f < n_frames; ++f) {
+    if (out_capacities[f] / std::max<uint32_t>(info.point_step, 1u) < (frame_points ? frame_points[f] : wh)) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+  }
   FrameChunks fc;
   if (int rc = fc.init(info, n_frames, frame_points)) return rc;
+  for (size_t f = 0; !zstd && out_capacities && f < n_frames; ++f) {
+    if (out_capacities[f] < fc.points[f] * info.point_step) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+  }
   bool ok;
-  const size_t max_body = stage2_max_body(info, fc.max_points, &ok);
-  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
   const size_t chunk_worst = max_compressed_size(plain, std::min<size_t>(fc.max_points, kChunkPoints), false, &ok) + 64;
-  const size_t cap = std::min(max_body, chunk_worst);
-  const size_t slot = (cap + 15) & ~size_t(15);
+  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
+  // ZSTD: a chunk may decompress to max_body bytes (the host-pointer bound), but not beyond its slot
+  const size_t body_cap = zstd ? std::min(stage2_max_body(info, fc.max_points, &ok), chunk_worst) : chunk_worst;
+  const size_t slot = (body_cap + 15) & ~size_t(15);
   fc.place(slot);
   const size_t chunks = fc.chunks;
   if (chunks > 0x7FFFFFFFull || slot > 0xFFFFFFF0ull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-  for (size_t f = 0; f < n_frames; ++f) {  // a frame without points has no chunk to decompress
+  for (size_t f = 0; zstd && f < n_frames; ++f) {  // a frame without points has no chunk to decompress
     if (fc.frame_chunks(f) == 0 && payload_bytes[f] != 0) { set_error("%s", dev_error_text(DEV_ERR_CHUNK_COUNT)); return CLDN_ERR_CORRUPT_DATA; }
   }
-  // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
-  const uint32_t wpc = zstd_warps_per_cta();
-  const size_t ctas = std::max<size_t>(1, std::min<size_t>((chunks + wpc - 1) / wpc, 2048 / wpc));
-  const size_t lit_stride = zstd_lit_scratch_bytes(static_cast<uint32_t>(cap));
+  size_t ctas = 0, lit_bytes = 0;
+  if (zstd) {  // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
+    const uint32_t wpc = zstd_warps_per_cta();
+    ctas = std::max<size_t>(1, std::min<size_t>((chunks + wpc - 1) / wpc, 2048 / wpc));
+    lit_bytes = ctas * wpc * zstd_lit_scratch_bytes(static_cast<uint32_t>(body_cap));
+  }
   if (int rc = d->d_s1.reserve(std::max<size_t>(fc.arena, 256))) return rc;
   if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
-  if (int rc = d->d_zs_lit.reserve(ctas * wpc * lit_stride)) return rc;
+  if (int rc = zstd ? d->d_zs_lit.reserve(lit_bytes) : CLDN_OK) return rc;
   if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
   if (int rc = d->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
   if (int rc = d->d_lz_frames.reserve(n_frames)) return rc;
@@ -1331,27 +1245,45 @@ static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n
   uint32_t* hcf = nullptr; int hcf_slot = 0;
   if (int rc = d->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
   if (int rc = d->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
-  fill_stage2_frames(d->d_s1.p, fc, n_frames, payloads, payload_bytes, hf, hcf);
+  uint32_t cb = 0;
+  for (size_t f = 0; f < n_frames; ++f) {
+    Lz4Frame& F = hf[f];
+    memset(&F, 0, sizeof(F));
+    F.packed_in = static_cast<const uint8_t*>(payloads[f]);
+    F.packed_in_bytes = payload_bytes[f];
+    F.plain_out = d->d_s1.p + fc.s1_off[f];
+    F.plain_cap = fc.s1_cap[f];
+    F.n_chunks = static_cast<uint32_t>(fc.frame_chunks(f));
+    F.chunk_begin = cb;
+    for (uint32_t c = 0; c < F.n_chunks; ++c) hcf[cb + c] = static_cast<uint32_t>(f);
+    cb += F.n_chunks;
+  }
   CUDA_TRY(cudaMemcpyAsync(d->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_lz_frames.commit(hf_slot, d->stream)) return rc;
   if (chunks) CUDA_TRY(cudaMemcpyAsync(d->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_lz_chunk_frame.commit(hcf_slot, d->stream)) return rc;
-  ZstdLaunch Z;
-  memset(&Z, 0, sizeof(Z));
-  Z.L.frames = d->d_lz_frames.p;
-  Z.L.n_frames = static_cast<uint32_t>(n_frames);
-  Z.L.n_chunks_total = static_cast<uint32_t>(chunks);
-  Z.L.chunk_frame = d->d_lz_chunk_frame.p;
-  Z.L.scratch = d->d_lz_scratch.p;
-  Z.L.slot_stride = static_cast<uint32_t>(slot);
-  Z.L.chunk_sizes = d->d_lz_chunk_sizes.p;
-  Z.L.sizes = d->d_lz_sizes.p;
-  Z.L.err = d->d_err.p;
-  Z.L.frame_err = d->frame_err;
-  Z.body_cap = static_cast<uint32_t>(cap);
-  Z.n_ctas = static_cast<uint32_t>(ctas);
-  Z.lit_scratch = d->d_zs_lit.p;
-  if (launch_zstd_decompress(Z, d->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  Lz4Launch L{};
+  L.frames = d->d_lz_frames.p;
+  L.n_frames = static_cast<uint32_t>(n_frames);
+  L.n_chunks_total = static_cast<uint32_t>(chunks);
+  L.chunk_frame = d->d_lz_chunk_frame.p;
+  L.scratch = d->d_lz_scratch.p;
+  L.slot_stride = static_cast<uint32_t>(slot);
+  L.chunk_sizes = d->d_lz_chunk_sizes.p;
+  L.sizes = d->d_lz_sizes.p;
+  L.err = d->d_err.p;
+  L.frame_err = d->frame_err;
+  if (zstd) {
+    ZstdLaunch Z{};
+    Z.L = L;
+    Z.body_cap = static_cast<uint32_t>(body_cap);
+    Z.n_ctas = static_cast<uint32_t>(ctas);
+    Z.lit_scratch = d->d_zs_lit.p;
+    if (launch_zstd_decompress(Z, d->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  } else if (launch_lz4_decompress(L, d->stream) < 0) {
+    set_error("LZ4 kernel launch failed");
+    return CLDN_ERR_CUDA;
+  }
   CUDA_TRY(cudaMemcpyAsync(d->h_lz_sizes.p, d->d_lz_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, d->stream));
   if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged frames stop here
   p1.resize(n_frames);
@@ -1360,58 +1292,35 @@ static int zstd_stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n
   return CLDN_OK;
 }
 
-static int decode_batch_device_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
-                                    const uint64_t* frame_points = nullptr) {
-  const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
-  for (size_t f = 0; f < n_frames; ++f) {
-    const uint64_t n_points = frame_points ? frame_points[f] : wh;
-    if (out_capacities[f] / std::max<uint32_t>(info.point_step, 1u) < n_points) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-  }
-  std::vector<const void*> p1;
-  std::vector<size_t> b1;
-  if (int rc = zstd_stage2_device(d, info, n_frames, payloads, payload_bytes, p1, b1, frame_points)) return rc;
-  cldn_info_t plain = info;
-  plain.compression_opt = CLDN_COMP_NONE;
-  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities, frame_points);
+// The decoder writes only the declared field bytes: where the layout has padding, a staged output starts as the caller's
+// bytes, so that the padding comes back unchanged.
+static int stage_padding(const cldn_decoder* d, void* staged, const void* out, size_t bytes, cudaStream_t stream) {
+  if (d->has_padding && bytes) CUDA_TRY(cudaMemcpyAsync(staged, out, bytes, cudaMemcpyHostToDevice, stream));
+  return CLDN_OK;
 }
 
 // Host pointers, compression ZSTD: the payloads go up compressed, the device decompresses and decodes them, the points
 // come back (with the caller's padding bytes, like the uncompressed host path).
 static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                  const size_t* payload_bytes, void* const* outs, const uint64_t* frame_points = nullptr) {
-  size_t in_total = 0;
-  std::vector<size_t> in_off(n_frames);
+                                  const size_t* payload_bytes, void* const* outs, const uint64_t* frame_points) {
+  std::vector<void*> din;
+  if (int rc = stage_layout(d->d_in, n_frames, payload_bytes, din)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
-    in_off[f] = in_total;
-    in_total += (payload_bytes[f] + 255) & ~size_t(255);
-  }
-  if (int rc = d->d_in.reserve(in_total + 256)) return rc;
-  std::vector<const void*> din(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) {
-    din[f] = d->d_in.p + in_off[f];
-    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(d->d_in.p + in_off[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->stream));
+    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(din[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->stream));
   }
   std::vector<const void*> p1;
   std::vector<size_t> b1;
-  if (int rc = zstd_stage2_device(d, info, n_frames, din.data(), payload_bytes, p1, b1, frame_points)) return rc;
+  if (int rc = stage2_device(d, info, n_frames, din.data(), payload_bytes, nullptr, frame_points, p1, b1)) return rc;
   cldn_info_t plain = info;
   plain.compression_opt = CLDN_COMP_NONE;
   if (int rc = decoder_update_plan(d, plain)) return rc;
   const size_t wh = static_cast<size_t>(info.width) * info.height;
-  std::vector<size_t> caps(n_frames), out_off(n_frames);
-  size_t out_total = 0;
+  std::vector<size_t> caps(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) caps[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
+  std::vector<void*> dout;
+  if (int rc = stage_layout(d->d_out, n_frames, caps.data(), dout)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
-    caps[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
-    out_off[f] = out_total;
-    out_total += (caps[f] + 255) & ~size_t(255);
-  }
-  if (int rc = d->d_out.reserve(out_total + 256)) return rc;
-  std::vector<void*> dout(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) {
-    dout[f] = d->d_out.p + out_off[f];
-    // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
-    if (d->has_padding && caps[f]) CUDA_TRY(cudaMemcpyAsync(dout[f], outs[f], caps[f], cudaMemcpyHostToDevice, d->stream));
+    if (int rc = stage_padding(d, dout[f], outs[f], caps[f], d->stream)) return rc;
   }
   if (int rc = decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), dout.data(), caps.data(), frame_points)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
@@ -1423,44 +1332,70 @@ static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size
 // Host pointers, no stage 2. `frame_points` as decode_batch_device takes it.
 static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
-                                   const uint64_t* frame_points = nullptr) {
+                                   const uint64_t* frame_points) {
   if (int rc = decoder_update_plan(d, info)) return rc;
   const size_t wh = static_cast<size_t>(info.width) * info.height;
-  size_t in_total = 0, out_total = 0;
-  std::vector<size_t> in_off(n_frames), out_need(n_frames), out_off(n_frames);
+  std::vector<size_t> out_need(n_frames);
   for (size_t f = 0; f < n_frames; ++f) {
     out_need[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
     if (out_capacities[f] < out_need[f]) { set_error("Output buffer is too small to hold the decoded data"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-    in_off[f] = in_total;
-    in_total += (payload_bytes[f] + 255) & ~size_t(255);
-    out_off[f] = out_total;
-    out_total += (out_need[f] + 255) & ~size_t(255);
   }
-  if (int rc = d->d_in.reserve(in_total + 256)) return rc;
-  if (int rc = d->d_out.reserve(out_total + 256)) return rc;
+  std::vector<void*> din, dout;
+  if (int rc = stage_layout(d->d_in, n_frames, payload_bytes, din)) return rc;
+  if (int rc = stage_layout(d->d_out, n_frames, out_need.data(), dout)) return rc;
   if (int rc = d->pipe.ensure(2 * n_frames)) return rc;
   // frame f: upload on the h2d stream -> decode on the handle's stream -> download on the d2h stream
   for (size_t f = 0; f < n_frames; ++f) {
-    const void* din = d->d_in.p + in_off[f];
-    void* dout = d->d_out.p + out_off[f];
-    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(d->d_in.p + in_off[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->pipe.h2d));
-    // only declared field bytes are written by the decoder: keep the caller's padding bytes intact
-    if (d->has_padding && out_need[f]) CUDA_TRY(cudaMemcpyAsync(dout, outs[f], out_need[f], cudaMemcpyHostToDevice, d->pipe.h2d));
+    if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(din[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->pipe.h2d));
+    if (int rc = stage_padding(d, dout[f], outs[f], out_need[f], d->pipe.h2d)) return rc;
     CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f], d->pipe.h2d));
     CUDA_TRY(cudaStreamWaitEvent(d->stream, d->pipe.ev[2 * f], 0));
     const uint64_t* pts = frame_points ? frame_points + f : nullptr;
     uint32_t* const group_err = d->frame_err;
     if (group_err) d->frame_err = group_err + f;  // one launch per frame: frame 0 of that launch is frame f of the group
-    const int rc = decode_batch_device(d, info, 1, &din, &payload_bytes[f], &dout, &out_need[f], pts);
+    const int rc = decode_batch_device(d, info, 1, &din[f], &payload_bytes[f], &dout[f], &out_need[f], pts);
     d->frame_err = group_err;
     if (rc) return rc;
     CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f + 1], d->stream));
     CUDA_TRY(cudaStreamWaitEvent(d->pipe.d2h, d->pipe.ev[2 * f + 1], 0));
-    if (out_need[f]) CUDA_TRY(cudaMemcpyAsync(outs[f], dout, out_need[f], cudaMemcpyDeviceToHost, d->pipe.d2h));
+    if (out_need[f]) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], out_need[f], cudaMemcpyDeviceToHost, d->pipe.d2h));
   }
   CUDA_TRY(cudaStreamSynchronize(d->pipe.d2h));
   // a failed decode must not hand back garbage silently: the error word is checked after everything has drained
   return check_device_error(d->stream, d->d_err.p, d->h_err.p);
+}
+
+// Whether decode_frames decodes frames of `info` in `mem` whole, with an error word per frame (DecLaunch /
+// Lz4Launch::frame_err). The others go frame by frame: LZ4 with host pointers and CLDN_B200_ZSTD_HOST through the host
+// libraries (decode_batch_impl), and compressions that no route decodes.
+static bool route_has_frame_errors(int mem, const cldn_info_t& info) {
+  switch (info.compression_opt) {
+    case CLDN_COMP_NONE: return true;
+    case CLDN_COMP_LZ4: return mem == CLDN_MEM_DEVICE;
+    case CLDN_COMP_ZSTD: return mem == CLDN_MEM_DEVICE || !zstd_host_route();
+    default: return false;
+  }
+}
+
+// Frames that share `info`, each with frame_points[f] points (nullptr: info.width * info.height), through the one route
+// of their memory kind and compression: device NONE, LZ4 or ZSTD (stage 2 then one fused stage-1 launch), host plain, or
+// host ZSTD decompressed on the device. Device routes leave the error word to the caller; host routes check it.
+static int decode_frames(cldn_decoder* d, int mem, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
+                         const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
+                         const uint64_t* frame_points) {
+  if (mem == CLDN_MEM_HOST) {
+    if (info.compression_opt == CLDN_COMP_ZSTD) return decode_batch_host_zstd(d, info, n_frames, payloads, payload_bytes, outs, frame_points);
+    return decode_batch_host_plain(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, frame_points);
+  }
+  if (info.compression_opt != CLDN_COMP_LZ4 && info.compression_opt != CLDN_COMP_ZSTD) {
+    return decode_batch_device(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, frame_points);
+  }
+  std::vector<const void*> p1;
+  std::vector<size_t> b1;
+  if (int rc = stage2_device(d, info, n_frames, payloads, payload_bytes, out_capacities, frame_points, p1, b1)) return rc;
+  cldn_info_t plain = info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, out_capacities, frame_points);
 }
 
 static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t n_frames, const void* const* payloads,
@@ -1472,13 +1407,7 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
   if (n_frames == 0) return CLDN_OK;
   CUDA_TRY(cudaSetDevice(d->device));
   if (mem == CLDN_MEM_DEVICE) {
-    if (info->compression_opt == CLDN_COMP_LZ4) {
-      if (int rc = decode_batch_device_lz4(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) return rc;
-    } else if (info->compression_opt == CLDN_COMP_ZSTD) {
-      if (int rc = decode_batch_device_zstd(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) return rc;
-    } else if (int rc = decode_batch_device(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities)) {
-      return rc;
-    }
+    if (int rc = decode_frames(d, mem, *info, n_frames, payloads, payload_bytes, outs, out_capacities, nullptr)) return rc;
     if (sync) return check_device_error(d->stream, d->d_err.p, d->h_err.p);
     return CLDN_OK;
   }
@@ -1507,16 +1436,17 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
     }
     const size_t max_body = stage2_max_body(*info, pts, &ok);
     if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-    if (device_zstd) return decode_batch_host_zstd(d, *info, n_frames, payloads, payload_bytes, outs);
-    for (size_t f = 0; f < n_frames; ++f) {
-      if (int rc = stage2_decompress_payload(info->compression_opt, static_cast<const uint8_t*>(payloads[f]), payload_bytes[f], d->s2_tmp, max_body)) return rc;
-      const void* p1 = d->s2_tmp.data();
-      const size_t b1 = d->s2_tmp.size();
-      if (int rc = decode_batch_impl(d, &plain, 1, &p1, &b1, &outs[f], &out_capacities[f], CLDN_MEM_HOST, 1)) return rc;
+    if (!device_zstd) {  // the host library, frame by frame
+      for (size_t f = 0; f < n_frames; ++f) {
+        if (int rc = stage2_decompress_payload(info->compression_opt, static_cast<const uint8_t*>(payloads[f]), payload_bytes[f], d->s2_tmp, max_body)) return rc;
+        const void* p1 = d->s2_tmp.data();
+        const size_t b1 = d->s2_tmp.size();
+        if (int rc = decode_batch_impl(d, &plain, 1, &p1, &b1, &outs[f], &out_capacities[f], CLDN_MEM_HOST, 1)) return rc;
+      }
+      return CLDN_OK;
     }
-    return CLDN_OK;
   }
-  return decode_batch_host_plain(d, *info, n_frames, payloads, payload_bytes, outs, out_capacities);
+  return decode_frames(d, mem, *info, n_frames, payloads, payload_bytes, outs, out_capacities, nullptr);
 }
 
 // ---- complete blobs, any mix of layouts and sizes (cldn_b200_decode_blobs) -----------------------------------------
@@ -1622,18 +1552,9 @@ static int decode_blob_group(cldn_decoder* d, int mem, const cldn_info_t& info, 
   if (int rc = d->h_frame_err.reserve(n)) return rc;
   CUDA_TRY(cudaMemsetAsync(d->d_frame_err.p, 0, n * sizeof(uint32_t), d->stream));
   d->frame_err = d->d_frame_err.p;
-  const int rc = [&]() -> int {
-    if (mem == CLDN_MEM_HOST) {
-      if (info.compression_opt == CLDN_COMP_ZSTD) return decode_batch_host_zstd(d, info, n, payloads, payload_bytes, outs, points);
-      return decode_batch_host_plain(d, info, n, payloads, payload_bytes, outs, caps, points);
-    }
-    int r;
-    if (info.compression_opt == CLDN_COMP_LZ4) r = decode_batch_device_lz4(d, info, n, payloads, payload_bytes, outs, caps, points);
-    else if (info.compression_opt == CLDN_COMP_ZSTD) r = decode_batch_device_zstd(d, info, n, payloads, payload_bytes, outs, caps, points);
-    else r = decode_batch_device(d, info, n, payloads, payload_bytes, outs, caps, points);
-    if (r) return r;
-    return check_device_error(d->stream, d->d_err.p, d->h_err.p);  // the launch word: errors no frame claimed
-  }();
+  int rc = decode_frames(d, mem, info, n, payloads, payload_bytes, outs, caps, points);
+  // the launch word: errors no frame claimed (the host routes have checked it)
+  if (rc == CLDN_OK && mem == CLDN_MEM_DEVICE) rc = check_device_error(d->stream, d->d_err.p, d->h_err.p);
   d->frame_err = nullptr;
   if (rc) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->h_frame_err.p, d->d_frame_err.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, d->stream));
@@ -1686,11 +1607,8 @@ static int decode_blobs_impl(cldn_decoder* d, size_t n, const void* const* blobs
     payload[f] = static_cast<const uint8_t*>(blobs[f]) + hdr[f];
     payload_bytes[f] = blob_bytes[f] - hdr[f];
     points[f] = static_cast<uint64_t>(I.width) * I.height;
-    alone[f] = I.version < 3 || I.compression_opt > CLDN_COMP_ZSTD || points[f] > 0xFFFFFFFFull || points[f] * I.point_step > caps[f];
-    if (mem == CLDN_MEM_HOST) {
-      alone[f] |= I.compression_opt == CLDN_COMP_LZ4 || (I.compression_opt == CLDN_COMP_ZSTD && zstd_host_route()) ||
-                  (payload_bytes[f] >= 10 && memcmp(payload[f], "CLOUDINI_V", 10) == 0);
-    }
+    alone[f] = !route_has_frame_errors(mem, I) || I.version < 3 || points[f] > 0xFFFFFFFFull || points[f] * I.point_step > caps[f] ||
+               (mem == CLDN_MEM_HOST && payload_bytes[f] >= 10 && memcmp(payload[f], "CLOUDINI_V", 10) == 0);
   }
   std::vector<size_t> members;
   std::vector<const void*> g_payload;

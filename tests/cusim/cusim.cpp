@@ -149,26 +149,27 @@ typedef std::mutex HostLock;
 namespace {
 
 HostLock g_pool_mutex;
-// CTA contexts (fiber stacks) are recycled between the launches of one host thread (its worker threads are created and
-// joined by it, which orders the reuse; sharing them between host threads would order those threads)
+// CTA contexts (fiber stacks) are recycled between the launches of one host thread. The host thread takes them from its
+// pool before it creates the launch's worker threads and returns them after it has joined them, so every reuse is
+// ordered by that join and the next create. A worker must not return its context itself: on a busy machine a sibling
+// worker of the same launch could start after that and take it, unordered. Sharing contexts between host threads would
+// order those threads.
 std::map<std::thread::id, std::vector<Cta*>> g_pool;
 
 Cta* acquire_cta(std::thread::id host) {
   {
     std::lock_guard<HostLock> lock(g_pool_mutex);
     std::vector<Cta*>& pool = g_pool[host];
-    if (!pool.empty()) { Cta* c = pool.back(); pool.pop_back(); g_cta = c; return c; }
+    if (!pool.empty()) { Cta* c = pool.back(); pool.pop_back(); return c; }
   }
   Cta* c = new Cta();
   c->stacks = static_cast<char*>(mmap(nullptr, kStackBytes * kMaxThreads, PROT_READ | PROT_WRITE,
                                       MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0));
   if (c->stacks == MAP_FAILED) { fprintf(stderr, "cusim: mmap of fiber stacks failed\n"); abort(); }
   for (unsigned i = 0; i < kMaxThreads; ++i) c->fibers[i].stack = c->stacks + kStackBytes * i;
-  g_cta = c;
   return c;
 }
 void release_cta(Cta* c, std::thread::id host) {
-  g_cta = nullptr;
   std::lock_guard<HostLock> lock(g_pool_mutex);
   g_pool[host].push_back(c);
 }
@@ -600,8 +601,8 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
   if (workers > 16) workers = 16;
   if (workers > n_ctas) workers = static_cast<unsigned>(n_ctas);
   std::atomic<uint64_t> next{0};
-  auto worker = [&]() {
-    Cta* c = acquire_cta(host);
+  auto worker = [&](Cta* c) {
+    g_cta = c;
     c->body = &body;
 #if CUSIM_ASAN
     // exactly the bytes the launch asked for (rounded to the 16-byte granularity the kernels' staged copies may read),
@@ -634,13 +635,16 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
                       static_cast<unsigned>(i / (static_cast<uint64_t>(grid.x) * grid.y))};
       run_cta(c, grid, block, bid);
     }
-    release_cta(c, host);
+    g_cta = nullptr;
   };
   // always on fresh OS threads: the caller's thread keeps its own (possibly small) stack out of the picture
+  std::vector<Cta*> ctas(workers);
+  for (Cta*& c : ctas) c = acquire_cta(host);
   std::vector<std::thread> pool;
   pool.reserve(workers);
-  for (unsigned w = 0; w < workers; ++w) pool.emplace_back(worker);
+  for (unsigned w = 0; w < workers; ++w) pool.emplace_back(worker, ctas[w]);
   for (auto& t : pool) t.join();
+  for (Cta* c : ctas) release_cta(c, host);
 }
 
 }  // namespace cusim
