@@ -14,7 +14,7 @@ from __future__ import annotations
 import ctypes as C
 import enum
 import os
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import List, Optional, Sequence
 
 __all__ = [
@@ -136,6 +136,8 @@ def lib():
     L.cldn_b200_encode.argtypes = [vp, vp, sz, vp, sz, C.c_int, C.POINTER(sz), C.c_int]
     L.cldn_b200_encode_batch.argtypes = [vp, sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.c_int,
                                          C.POINTER(sz), C.c_int]
+    L.cldn_b200_encode_blobs.argtypes = [vp, sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                         C.POINTER(vp), C.POINTER(sz), C.POINTER(sz), C.c_int]
     L.cldn_b200_encoder_sizes_device.argtypes = [vp]
     L.cldn_b200_encoder_sizes_device.restype = vp
     L.cldn_b200_encoder_sync.argtypes = [vp]
@@ -345,6 +347,52 @@ class PointcloudEncoder:
         written = (C.c_size_t * n)() if want_sizes else None
         _check(lib().cldn_b200_encode_batch(self._h, n, a_in, a_inb, a_out, a_cap, 1 if write_header else 0, written, MEM_DEVICE))
         return list(written) if want_sizes else None
+
+    @staticmethod
+    def _dims(n: int, dims):
+        """(widths, heights) ctypes arrays for encode_blobs: None for width = points, height = 1."""
+        if dims is None:
+            return None, None
+        if len(dims) != n:
+            raise RuntimeError("dims must have one (width, height) per frame")
+        m = max(n, 1)
+        return (C.c_uint32 * m)(*[int(w) for w, _ in dims]), (C.c_uint32 * m)(*[int(h) for _, h in dims])
+
+    def encode_blobs(self, clouds: Sequence, dims: Optional[Sequence] = None) -> List[bytes]:
+        """Complete blobs of host clouds of this encoder's layout, each with a header stating its own dims: ``dims`` is
+        one (width, height) per cloud, or None for (points, 1). Blob f equals what set_dims(w_f, h_f) + encode(cloud_f)
+        give; this encoder's header is not changed."""
+        import numpy as np
+        n = len(clouds)
+        m = max(n, 1)
+        step = self._info.point_step
+        widths, heights = self._dims(n, dims)
+        ins = [_host_ptr(c) for c in clouds]
+        caps = []
+        for k, (_, nbytes, _) in enumerate(ins):
+            pts = nbytes // step if step else 0
+            w, h = dims[k] if dims is not None else (pts, 1)
+            # a cloud that is not a whole number of points gets a 1-byte buffer: the library reports the frame
+            caps.append(MaxCompressedSize(replace(self._info, width=int(w), height=int(h)), pts, True) if step and nbytes % step == 0 else 1)
+        outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps]
+        written = (C.c_size_t * m)()
+        _check(lib().cldn_b200_encode_blobs(self._h, n, (C.c_void_p * m)(*[p[0] for p in ins]), (C.c_size_t * m)(*[p[1] for p in ins]),
+                                            widths, heights, (C.c_void_p * m)(*[o.ctypes.data for o in outs]), (C.c_size_t * m)(*caps),
+                                            written, MEM_HOST))
+        del ins
+        return [outs[f][:written[f]].tobytes() for f in range(n)]
+
+    def encode_blobs_device(self, in_ptrs: Sequence[int], in_bytes: Sequence[int], out_ptrs: Sequence[int], out_caps: Sequence[int],
+                            dims: Optional[Sequence] = None, want_sizes: bool = True):
+        """encode_blobs for device-resident clouds and outputs (device addresses). Returns the blob sizes, or None when
+        want_sizes is False: the call is then asynchronous and the sizes stay at sizes_device_ptr()."""
+        n = len(in_ptrs)
+        m = max(n, 1)
+        widths, heights = self._dims(n, dims)
+        written = (C.c_size_t * m)() if want_sizes else None
+        _check(lib().cldn_b200_encode_blobs(self._h, n, (C.c_void_p * m)(*in_ptrs), (C.c_size_t * m)(*in_bytes), widths, heights,
+                                            (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps), written, MEM_DEVICE))
+        return [int(written[f]) for f in range(n)] if want_sizes else None
 
     def sizes_device_ptr(self) -> int:
         return int(lib().cldn_b200_encoder_sizes_device(self._h) or 0)

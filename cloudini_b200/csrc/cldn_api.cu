@@ -315,6 +315,9 @@ struct cldn_encoder {
   DevBuf<Lz4Frame> d_lz_frames;
   PinRing<Lz4Frame> h_lz_frames;
   PinRing<uint32_t> h_lz_chunk_frame;
+  // cldn_b200_encode_blobs: blob addresses, header offsets and the packed headers of a batch (launch_place_headers)
+  DevBuf<uint8_t> d_blob_headers;
+  PinRing<uint8_t> h_blob_headers;
 };
 
 // LZ4_COMPRESSBOUND (lz4.h): worst case of a block for n input bytes
@@ -841,6 +844,98 @@ int cldn_b200_encode(cldn_encoder_t* enc, const void* cloud, size_t cloud_bytes,
   const void* clouds[1] = {cloud};
   void* outs[1] = {out};
   return cldn_b200_encode_batch(enc, 1, clouds, &cloud_bytes, outs, &out_capacity, write_header, written, mem);
+}
+
+}  // extern "C"
+
+// Complete blobs of frames with their own dims: each frame's header is made on the host, the payloads are encoded by the
+// batch paths behind it (write_header = 0), and the headers are put in front of them afterwards (device pointers: one
+// launch that also turns the payload sizes into blob sizes; host pointers: memcpy). The handle's header is not touched.
+static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                             const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
+                             size_t* written_host, int mem) {
+  if (!e || (n_frames && (!clouds || !cloud_bytes || !outs || !out_capacities))) {
+    set_error("null argument");
+    return CLDN_ERR_INVALID_ARGUMENT;
+  }
+  if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n_frames == 0) return CLDN_OK;
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && e->stage2 != CLDN_COMP_LZ4) {
+    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
+    return CLDN_ERR_UNSUPPORTED;
+  }
+  if (mem == CLDN_MEM_HOST && e->stage2 != CLDN_COMP_NONE && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
+  cldn_info_t full = e->info;
+  full.compression_opt = static_cast<uint8_t>(e->stage2);
+  std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
+  std::vector<uint64_t> at(n_frames + 1, 0);
+  std::vector<void*> payload(n_frames);
+  std::vector<size_t> payload_cap(n_frames);
+  auto frame_error = [](size_t f, int rc) {
+    const std::string msg = cldn_b200_last_error();
+    set_error("frame %zu: %s", f, msg.c_str());
+    return rc;
+  };
+  for (size_t f = 0; f < n_frames; ++f) {
+    const size_t n = full.point_step ? cloud_bytes[f] / full.point_step : 0;
+    cldn_info_t fi = full;
+    fi.width = widths ? widths[f] : static_cast<uint32_t>(n);
+    fi.height = heights ? heights[f] : 1u;
+    const std::vector<uint8_t> h = make_header(fi);
+    size_t need;
+    if (int rc = check_encode_frame(full, h.size(), cloud_bytes[f], out_capacities[f], &need)) return frame_error(f, rc);
+    if (n > 0xFFFFFFFFull) { set_error("too many points in one frame"); return frame_error(f, CLDN_ERR_UNSUPPORTED); }
+    if (static_cast<uint64_t>(fi.width) * fi.height != n) {
+      set_error("width * height (%u x %u) differs from the %zu points of the cloud", fi.width, fi.height, n);
+      return frame_error(f, CLDN_ERR_INVALID_ARGUMENT);
+    }
+    if (!outs[f] || (n > 0 && !clouds[f])) { set_error("null frame pointer"); return frame_error(f, CLDN_ERR_INVALID_ARGUMENT); }
+    headers.insert(headers.end(), h.begin(), h.end());
+    at[f + 1] = headers.size();
+    payload[f] = static_cast<uint8_t*>(outs[f]) + h.size();
+    payload_cap[f] = out_capacities[f] - h.size();
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  if (mem == CLDN_MEM_HOST) {
+    std::vector<size_t> w(n_frames, 0);
+    if (int rc = encode_batch_impl(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data(), mem)) return rc;
+    for (size_t f = 0; f < n_frames; ++f) {
+      memcpy(outs[f], headers.data() + at[f], at[f + 1] - at[f]);
+      if (written_host) written_host[f] = (at[f + 1] - at[f]) + w[f];
+    }
+    return CLDN_OK;
+  }
+  const int rc = e->stage2 == CLDN_COMP_LZ4
+                     ? encode_batch_device_lz4(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0)
+                     : encode_batch_device(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0);
+  if (rc) return rc;
+  const size_t tab_bytes = (2 * n_frames + 1) * sizeof(uint64_t) + headers.size();
+  uint8_t* ht = nullptr;
+  int slot = 0;
+  if (int rc2 = e->h_blob_headers.acquire(tab_bytes, &ht, &slot)) return rc2;
+  if (int rc2 = e->d_blob_headers.reserve(tab_bytes)) return rc2;
+  uint64_t* tab = reinterpret_cast<uint64_t*>(ht);
+  for (size_t f = 0; f < n_frames; ++f) tab[f] = reinterpret_cast<uintptr_t>(outs[f]);
+  memcpy(tab + n_frames, at.data(), (n_frames + 1) * sizeof(uint64_t));
+  memcpy(tab + 2 * n_frames + 1, headers.data(), headers.size());
+  CUDA_TRY(cudaMemcpyAsync(e->d_blob_headers.p, ht, tab_bytes, cudaMemcpyHostToDevice, e->stream));
+  if (int rc2 = e->h_blob_headers.commit(slot, e->stream)) return rc2;
+  if (launch_place_headers(reinterpret_cast<const uint64_t*>(e->d_blob_headers.p), static_cast<uint32_t>(n_frames), e->d_sizes.p,
+                           e->stream) < 0) {
+    set_error("header launch failed");
+    return CLDN_ERR_CUDA;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return read_written(e, n_frames, written_host);
+}
+
+extern "C" {
+
+int cldn_b200_encode_blobs(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                           const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
+                           size_t* written_host, int mem) {
+  return guarded([&] { return encode_blobs_impl(e, n_frames, clouds, cloud_bytes, widths, heights, outs, out_capacities, written_host, mem); });
 }
 
 }  // extern "C"

@@ -42,6 +42,8 @@ def _L():
         L.cldn_b200_preproc_destroy.argtypes = [vp]
         L.cldn_b200_preproc_destroy.restype = None
         L.cldn_b200_viz_lossy_preprocess.argtypes = [vp, C.POINTER(_CInfo), vp, sz, vp, sz, C.POINTER(sz), C.POINTER(C.c_int), C.c_int]
+        L.cldn_b200_viz_lossy_preprocess_batch.argtypes = [vp, C.POINTER(_CInfo), sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp),
+                                                           C.POINTER(sz), C.POINTER(sz), C.POINTER(C.c_int), C.POINTER(_CInfo), C.c_int]
         L.cldn_b200_ros_parse.argtypes = [vp, sz, C.POINTER(_CRosMsg)]
         L.cldn_b200_ros_to_encoding_info.argtypes = [C.POINTER(_CRosMsg), C.POINTER(_CInfo)]
         L.cldn_b200_ros_apply_resolution_profile.argtypes = [C.POINTER(_CField), C.POINTER(C.c_uint32), C.POINTER(C.c_char_p),
@@ -252,6 +254,38 @@ class VizPreprocessor:
         _check(_L().cldn_b200_viz_lossy_preprocess(self._h, C.byref(c), C.c_void_p(in_ptr), nbytes, C.c_void_p(out_ptr), out_capacity,
                                                    C.byref(kept), C.byref(applied), MEM_DEVICE))
         return (_from_c(c) if applied.value else info), kept.value, bool(applied.value)
+
+    def _batch(self, info: EncodingInfo, n: int, in_ptrs, in_bytes, out_ptrs, out_caps, mem: int):
+        m = max(n, 1)
+        c = _to_c(info)
+        kept, applied, infos = (C.c_size_t * m)(), (C.c_int * m)(), (_CInfo * m)()
+        _check(_L().cldn_b200_viz_lossy_preprocess_batch(self._h, C.byref(c), n, (C.c_void_p * m)(*in_ptrs), (C.c_size_t * m)(*in_bytes),
+                                                         (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps), kept, applied,
+                                                         infos, mem))
+        out = []
+        for f in range(n):
+            new_info = info
+            if applied[f]:
+                new_info = _from_c(infos[f])
+                new_info.use_threads = info.use_threads
+            out.append((new_info, int(kept[f]), bool(applied[f])))
+        return out
+
+    def run_batch(self, info: EncodingInfo, clouds):
+        """``run`` for a list of host clouds of one layout, in one launch pair: returns one (new_info, survivors as a uint8
+        array, applied) per cloud, with run's no-op convention (the input array and ``info`` when not applied)."""
+        arrs = [np.frombuffer(c, dtype=np.uint8) if isinstance(c, (bytes, bytearray, memoryview))
+                else np.ascontiguousarray(c).view(np.uint8).reshape(-1) for c in clouds]
+        outs = [np.zeros(max(a.size, 1), dtype=np.uint8) for a in arrs]
+        res = self._batch(info, len(arrs), [a.ctypes.data if a.size else None for a in arrs], [a.size for a in arrs],
+                          [o.ctypes.data for o in outs], [o.size for o in outs], MEM_HOST)
+        return [(new_info, outs[f][:kept * info.point_step] if applied else arrs[f], applied)
+                for f, (new_info, kept, applied) in enumerate(res)]
+
+    def run_batch_device(self, info: EncodingInfo, in_ptrs, in_bytes, out_ptrs, out_caps):
+        """Device-pointer variant of run_batch: returns one (new_info, kept_points, applied) per cloud; survivors are at
+        out_ptrs[f]."""
+        return self._batch(info, len(in_ptrs), in_ptrs, in_bytes, out_ptrs, out_caps, MEM_DEVICE)
 
 
 def applyVizLossyPreprocessing(pc: RosPointCloud2, preprocessor: Optional[VizPreprocessor] = None) -> None:

@@ -150,6 +150,19 @@ int cldn_b200_encode(cldn_encoder_t* enc, const void* cloud, size_t cloud_bytes,
 int cldn_b200_encode_batch(cldn_encoder_t* enc, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                            void* const* outs, const size_t* out_capacities, int write_header, size_t* written_host,
                            int mem);
+/* Batch of frames of this encoder's layout, each written as a complete blob whose header states the frame's own
+ * width / height (no reference counterpart: the reference builds a PointcloudEncoder per message). Blob f is
+ * byte-identical to cldn_b200_encoder_set_dims(enc, widths[f], heights[f]) + cldn_b200_encode(..., write_header = 1)
+ * with this handle. widths and heights are both NULL (width = point count, height = 1) or both given, with
+ * widths[f] * heights[f] equal to frame f's point count. Every frame is checked before anything launches, in the order
+ * of cldn_b200_encode with that frame's header length; the first bad frame's status is returned with
+ * "frame <f>: <message>" and no output byte is written. Memory kinds, compression options and their refusals are those of
+ * cldn_b200_encode_batch; with CLDN_MEM_DEVICE and written_host == NULL the call is asynchronous, and
+ * cldn_b200_encoder_sizes_device then holds the blob sizes, headers included. The handle's header and dims are unchanged.
+ * Device pointers: the encode_batch launches plus one launch that puts the headers in front of the payloads. */
+int cldn_b200_encode_blobs(cldn_encoder_t* enc, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                           const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
+                           size_t* written_host, int mem);
 /* Device array (uint64 per frame of the last batch) with the encoded sizes; valid after the stream is synchronised. */
 const uint64_t* cldn_b200_encoder_sizes_device(const cldn_encoder_t* enc);
 /* Re-uses an encoder for messages of the same layout but another width / height (no reference counterpart: the

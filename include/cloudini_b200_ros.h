@@ -37,6 +37,19 @@ void cldn_b200_preproc_destroy(cldn_preproc_t* pp);
 int cldn_b200_viz_lossy_preprocess(cldn_preproc_t* pp, cldn_info_t* info, const void* cloud, size_t cloud_bytes,
                                    void* out, size_t out_capacity, size_t* kept_points, int* applied, int mem);
 
+/* The same preprocessing for n_frames clouds of one layout `info` (no reference counterpart: the reference handles one
+ * message per call). Frame f's output bytes, kept_points[f], applied[f] and infos_out[f] (optional, n_frames entries) are
+ * what cldn_b200_viz_lossy_preprocess gives that cloud alone, `info` in and out being infos_out[f]: a layout without the
+ * triple or with a bad resolution makes every frame a no-op, an empty cloud only its own frame (applied[f] = 0, output
+ * untouched, infos_out[f] = *info). Every frame is checked before anything launches; the first bad frame's status is
+ * returned with "frame <f>: <message>". One insert and one compact launch cover all frames, followed by one read-back
+ * of the survivor counts and one synchronisation, for both memory kinds. Workspace: about 28 bytes per point of the
+ * batch, kept by the handle. */
+int cldn_b200_viz_lossy_preprocess_batch(cldn_preproc_t* pp, const cldn_info_t* info, size_t n_frames,
+                                         const void* const* clouds, const size_t* cloud_bytes, void* const* outs,
+                                         const size_t* out_capacities, size_t* kept_points, int* applied,
+                                         cldn_info_t* infos_out, int mem);
+
 /* ---- N2: DDS envelope ------------------------------------------------------------------------------------------- */
 /* Parsed view of a CDR-serialised sensor_msgs/msg/PointCloud2 or point_cloud_interfaces/msg/CompressedPointCloud2
  * (cloudini_ros::RosPointCloud2, ros_msg_utils.hpp:32-148). `frame_id` and `data` are views (into the message that was
