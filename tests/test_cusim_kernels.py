@@ -36,8 +36,10 @@ def _run_gpu_suite(cusim_lib, extra_env, selection):
 
 
 def test_parity_suite_under_emulation(cusim_lib):
-    out = _run_gpu_suite(cusim_lib, {"CLDN_B200_FUZZ": "1", "CLDN_B200_FUZZ_SEEDS": "60"}, ["tests/test_gpu_parity.py", "tests/test_gpu_fast_paths.py", "tests/test_gpu_stage2_device.py", "tests/test_gpu_ros.py",
-                                    "tests/test_gpu_zz_legacy_kernels.py", "tests/test_cpp_shim.py", "tests/test_gpu_concurrency.py"])
+    # test_gpu_zstd_format.py: the ZSTD decompressor through the product's C ABI on a small corpus (CLDN_ZSTD_FORMAT_SMALL)
+    out = _run_gpu_suite(cusim_lib, {"CLDN_B200_FUZZ": "1", "CLDN_B200_FUZZ_SEEDS": "60", "CLDN_ZSTD_FORMAT_SMALL": "1"},
+                         ["tests/test_gpu_parity.py", "tests/test_gpu_fast_paths.py", "tests/test_gpu_stage2_device.py", "tests/test_gpu_ros.py",
+                          "tests/test_gpu_zz_legacy_kernels.py", "tests/test_cpp_shim.py", "tests/test_gpu_concurrency.py", "tests/test_gpu_zstd_format.py"])
     assert " passed" in out and "failed" not in out
 
 

@@ -7,9 +7,10 @@ ZSTD_decompress(dst, cap, body, size), and fails exactly when ZSTD_decompress fa
 The corpus is compressed here with the system libzstd (ctypes) from stage-1 chunks of the C oracle: levels 1 / 3 / 19 / -5,
 a content checksum, no content size, streaming with a flush every few KB (many blocks per frame: treeless literals and
 repeat tables), a constant chunk, 0 / 1 / 3-point chunks, two frames with a skippable frame between them. A block-header
-inspector counts which format features the corpus exercises; the test fails if one of them is missing.
+inspector counts which format features the corpus exercises; the test fails if one of them is missing. The libzstd
+bindings, the hand-written frames, the inspector and the corruption live in tests/zstd_corpus.py, which
+tests/test_gpu_zstd_format.py shares to run the same format features through the product's API on the GPU.
 """
-import ctypes as C
 import os
 import platform
 import random
@@ -25,94 +26,9 @@ HERE = os.path.join(ROOT, "tests", "cusim")
 sys.path.insert(0, HERE)
 sys.path.insert(0, ROOT)
 
+from zstd_corpus import REQUIRED, _known_gap, compress, compress_flushing, damage, decompress, hand_frames, inspect, zstd_lib  # noqa: E402
+
 pytestmark = pytest.mark.skipif(platform.machine() != "x86_64", reason="cusim's context switch is x86-64 only")
-
-
-# ---- libzstd through ctypes ------------------------------------------------------------------------------------------
-class _In(C.Structure):
-    _fields_ = [("src", C.c_void_p), ("size", C.c_size_t), ("pos", C.c_size_t)]
-
-
-class _Out(C.Structure):
-    _fields_ = [("dst", C.c_void_p), ("size", C.c_size_t), ("pos", C.c_size_t)]
-
-
-def zstd_lib():
-    try:
-        z = C.CDLL("libzstd.so.1")
-    except OSError:
-        pytest.skip("libzstd.so.1 is not installed")
-    z.ZSTD_compress.restype = C.c_size_t
-    z.ZSTD_compress.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]
-    z.ZSTD_decompress.restype = C.c_size_t
-    z.ZSTD_decompress.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-    z.ZSTD_isError.restype = C.c_uint
-    z.ZSTD_isError.argtypes = [C.c_size_t]
-    z.ZSTD_compressBound.restype = C.c_size_t
-    z.ZSTD_compressBound.argtypes = [C.c_size_t]
-    z.ZSTD_createCCtx.restype = C.c_void_p
-    z.ZSTD_freeCCtx.argtypes = [C.c_void_p]
-    z.ZSTD_CCtx_setParameter.restype = C.c_size_t
-    z.ZSTD_CCtx_setParameter.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    z.ZSTD_compress2.restype = C.c_size_t
-    z.ZSTD_compress2.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-    z.ZSTD_compressStream2.restype = C.c_size_t
-    z.ZSTD_compressStream2.argtypes = [C.c_void_p, C.POINTER(_Out), C.POINTER(_In), C.c_int]
-    return z
-
-
-C_LEVEL, C_CONTENT_SIZE, C_CHECKSUM = 100, 200, 201
-E_CONTINUE, E_FLUSH, E_END = 0, 1, 2
-
-
-def compress(z, data: bytes, level=1, checksum=None, content_size=None) -> bytes:
-    cap = z.ZSTD_compressBound(len(data))
-    dst = C.create_string_buffer(cap)
-    if checksum is None and content_size is None:
-        r = z.ZSTD_compress(dst, cap, data, len(data), level)
-    else:
-        cc = z.ZSTD_createCCtx()
-        z.ZSTD_CCtx_setParameter(cc, C_LEVEL, level)
-        if checksum is not None:
-            z.ZSTD_CCtx_setParameter(cc, C_CHECKSUM, int(checksum))
-        if content_size is not None:
-            z.ZSTD_CCtx_setParameter(cc, C_CONTENT_SIZE, int(content_size))
-        r = z.ZSTD_compress2(cc, dst, cap, data, len(data))
-        z.ZSTD_freeCCtx(cc)
-    assert not z.ZSTD_isError(r)
-    return dst.raw[:r]
-
-
-def compress_flushing(z, data: bytes, level: int, every: int) -> bytes:
-    """Streaming compression with ZSTD_e_flush every `every` bytes: many blocks in one (windowed) frame."""
-    cc = z.ZSTD_createCCtx()
-    z.ZSTD_CCtx_setParameter(cc, C_LEVEL, level)
-    cap = z.ZSTD_compressBound(len(data)) + 64 * (len(data) // every + 2)
-    dst = C.create_string_buffer(cap)
-    src = C.create_string_buffer(data, len(data))
-    out = _Out(C.cast(dst, C.c_void_p), cap, 0)
-    for start in range(0, len(data) + 1, every):
-        end = min(start + every, len(data))
-        inp = _In(C.cast(src, C.c_void_p).value + start, end - start, 0)
-        op = E_END if end == len(data) else E_FLUSH
-        while True:
-            r = z.ZSTD_compressStream2(cc, C.byref(out), C.byref(inp), op)
-            assert not z.ZSTD_isError(r)
-            if r == 0 and inp.pos == inp.size:
-                break
-        if op == E_END:
-            break
-    z.ZSTD_freeCCtx(cc)
-    return dst.raw[:out.pos]
-
-
-def decompress(z, body: bytes, cap: int):
-    """(ok, bytes) of ZSTD_decompress(dst, cap, body, len(body))."""
-    dst = C.create_string_buffer(max(cap, 1))
-    r = z.ZSTD_decompress(dst, cap, body, len(body))
-    if z.ZSTD_isError(r):
-        return False, b""
-    return True, dst.raw[:r]
 
 
 # ---- corpus --------------------------------------------------------------------------------------------------------
@@ -140,32 +56,6 @@ def stage1_chunks():
         for k, c in enumerate(body[:2]):
             chunks[f"{name}_{k}"] = c
     return chunks
-
-
-def hand_frames():
-    """Frames libzstd's compressor does not write on its own: a 0-point chunk (empty body), a raw literals section with
-    a 2-byte count of 0 sequences, a 1-byte and a 4-byte content size, a dictionary-ID field of 0, and raw / RLE blocks
-    above the 128 KB block maximum (accepted by ZSTD_decompress)."""
-    def frame(fhd, extra, blocks):
-        return struct.pack("<I", 0xFD2FB528) + bytes([fhd]) + extra + b"".join(blocks)
-
-    def bh(last, btype, size):
-        v = (size << 3) | (btype << 1) | last
-        return struct.pack("<I", v)[:3]
-    raw = bytes(range(200))
-    out = {
-        "empty_body": b"",
-        "fcs1_raw": frame(0x20, bytes([200]), [bh(1, 0, 200) + raw]),                       # single segment, 1-byte FCS
-        "fcs4_did0": frame(0x81 | 0x20, bytes([0]) + struct.pack("<I", 200), [bh(1, 0, 200) + raw]),  # 1-byte DID 0, 4-byte FCS
-        "windowed_raw": frame(0x00, bytes([0x08]), [bh(0, 0, 100) + raw[:100], bh(1, 0, 100) + raw[100:]]),
-        # compressed block: raw literals (5 bytes) + a 2-byte sequence count of 0 (then the modes byte, predefined tables)
-        "nseq_long0": frame(0x20, bytes([5]), [bh(1, 2, 1 + 5 + 3) + bytes([5 << 3]) + b"abcde" + bytes([0x80, 0x00, 0x00])]),
-        # RLE literals: libzstd writes them only for a block whose > 63 literals are one byte value
-        "rle_literals": frame(0x20, bytes([20]), [bh(1, 2, 3) + bytes([(20 << 3) | 1, 0x41, 0])]),
-        "raw_200k": frame(0x00, bytes([0x30]), [bh(1, 0, 200_000) + bytes(random.Random(1).randbytes(200_000))]),
-        "rle_300k": frame(0x00, bytes([0x30]), [bh(1, 1, 300_000) + b"\x07"]),
-    }
-    return out
 
 
 def build_corpus(z):
@@ -201,80 +91,6 @@ def build_corpus(z):
     corpus["words_flush1k_L3"] = compress_flushing(z, b" ".join(rng.choice(words) for _ in range(12000)), 3, 1024)
     corpus.update(hand_frames())
     return corpus
-
-
-# ---- block-header inspector --------------------------------------------------------------------------------------------
-def inspect(body: bytes, feats: dict):
-    """Counts the format features of `body` (a valid ZSTD chunk body) into feats."""
-    def add(k):
-        feats[k] = feats.get(k, 0) + 1
-    pos = 0
-    while len(body) - pos >= 5:
-        (magic,) = struct.unpack_from("<I", body, pos)
-        if magic & 0xFFFFFFF0 == 0x184D2A50:
-            add("skippable_frame")
-            (sz,) = struct.unpack_from("<I", body, pos + 4)
-            pos += 8 + sz
-            continue
-        add("frame")
-        fhd = body[pos + 4]
-        single, fcs_code, did_code = (fhd >> 5) & 1, fhd >> 6, fhd & 3
-        add("single_segment" if single else "windowed_frame")
-        if fhd & 4:
-            add("checksum")
-        fcs_size = (single if fcs_code == 0 else 1 << fcs_code)
-        add(f"fcs_bytes_{fcs_size}")
-        p = pos + 5 + (0 if single else 1) + (0, 1, 2, 4)[did_code] + fcs_size
-        while True:
-            (h,) = struct.unpack_from("<I", body[p:p + 3] + b"\0")
-            last, btype, bsize = h & 1, (h >> 1) & 3, h >> 3
-            p += 3
-            add(("raw_block", "rle_block", "compressed_block")[btype])
-            if btype == 2:
-                blk = body[p:p + bsize]
-                lt, lhl = blk[0] & 3, (blk[0] >> 2) & 3
-                add(("raw_literals", "rle_literals", "huffman_literals", "treeless_literals")[lt])
-                if lt <= 1:
-                    lh = (1, 2, 1, 3)[lhl]
-                    lsz = (blk[0] >> 3) if lh == 1 else (struct.unpack_from("<H", blk)[0] >> 4 if lh == 2 else (blk[0] | blk[1] << 8 | blk[2] << 16) >> 4)
-                    used = lh + (lsz if lt == 0 else 1)
-                else:
-                    add("huffman_1_stream" if lhl == 0 else "huffman_4_streams")
-                    (lhc,) = struct.unpack_from("<I", blk)
-                    if lhl <= 1:
-                        lh, csz = 3, (lhc >> 14) & 0x3FF
-                    elif lhl == 2:
-                        lh, csz = 4, lhc >> 18
-                    else:
-                        lh, csz = 5, (lhc >> 22) + (blk[4] << 10)
-                    if lt == 2:
-                        add("huffman_weights_direct" if blk[lh] >= 128 else "huffman_weights_fse")
-                    used = lh + csz
-                ns = blk[used]
-                q = used + 1
-                if ns == 0:
-                    add("no_sequences")
-                else:
-                    if ns == 255:
-                        q += 2
-                    elif ns >= 128:
-                        q += 1
-                    modes = blk[q]
-                    for name, m in (("ll", modes >> 6), ("of", (modes >> 4) & 3), ("ml", (modes >> 2) & 3)):
-                        add(f"{name}_" + ("predefined", "rle", "fse", "repeat")[m])
-            p += 1 if btype == 1 else bsize
-            if last:
-                break
-        if fhd & 4:
-            p += 4
-        pos = p
-
-
-REQUIRED = ["frame", "skippable_frame", "single_segment", "windowed_frame", "checksum", "fcs_bytes_0", "fcs_bytes_1", "fcs_bytes_2",
-            "fcs_bytes_4", "raw_block", "rle_block", "compressed_block", "raw_literals", "rle_literals", "huffman_literals",
-            "treeless_literals", "huffman_1_stream", "huffman_4_streams", "huffman_weights_fse", "no_sequences",
-            "ll_predefined", "ll_rle", "ll_fse", "ll_repeat", "of_predefined", "of_rle", "of_fse", "of_repeat",
-            "ml_predefined", "ml_rle", "ml_fse", "ml_repeat"]
 
 
 # ---- the emulated kernel ---------------------------------------------------------------------------------------------
@@ -340,34 +156,6 @@ def cap_for(z, body):
     return max(len(data), 1) + 64 if ok else 1 << 20
 
 
-def damage(rng, body: bytes) -> bytes:
-    """One seeded corruption: bit flips, truncation, forged block size, forged table header bytes, appended bytes."""
-    b = bytearray(body)
-    kind = rng.randrange(6)
-    if not b:
-        return bytes([rng.randrange(256) for _ in range(rng.randrange(1, 12))])
-    if kind == 0:
-        for _ in range(rng.randrange(1, 4)):
-            i = rng.randrange(len(b))
-            b[i] ^= 1 << rng.randrange(8)
-    elif kind == 1:
-        del b[rng.randrange(len(b)):]
-    elif kind == 2 and len(b) > 12:   # block header: first block after a frame header of 5..14 bytes
-        i = rng.randrange(5, min(len(b) - 3, 18))
-        v = int.from_bytes(b[i:i + 3], "little") ^ (1 << rng.randrange(3, 24))
-        b[i:i + 3] = v.to_bytes(3, "little")
-    elif kind == 3 and len(b) > 20:   # bytes where literal / sequence / table headers sit
-        for _ in range(rng.randrange(1, 3)):
-            i = rng.randrange(5, min(len(b), 64))
-            b[i] = rng.randrange(256)
-    elif kind == 4 and len(b) > 8:    # the end of the sequence bitstream (offsets, lengths, final states)
-        i = len(b) - 1 - rng.randrange(min(len(b) - 1, 24))
-        b[i] ^= 1 << rng.randrange(8)
-    else:
-        b += bytes([rng.randrange(256) for _ in range(rng.randrange(1, 6))])
-    return bytes(b)
-
-
 @pytest.fixture(scope="module")
 def z():
     return zstd_lib()
@@ -411,16 +199,6 @@ def test_output_bound_is_the_capacity(z, corpus, driver, tmp_path):
     got, _ = run_kernel(driver, cases, tmp_path)
     for (cap, body), res in zip(cases, got):
         assert res == decompress(z, body, cap), cap
-
-
-def _known_gap(body, res, want):
-    """The one documented difference (see the damaged-frames test): accepted here, refused by libzstd, 4 Huffman streams."""
-    feats = {}
-    try:
-        inspect(body, feats)
-    except (IndexError, struct.error):
-        pass
-    return res[0] and not want[0] and bool(feats.get("huffman_4_streams"))
 
 
 def _damaged_cases(z, corpus, count, seed):
