@@ -31,20 +31,18 @@ def needs_build():
     return any(os.path.getmtime(os.path.join(CSRC, f)) > t for f in SOURCES + HEADERS)
 
 
-def build(force=False, verbose=False, defines=(), out=None):
-    """Compile every translation unit for sm_90a and link the shared library. Returns the library path.
-    `defines` / `out` build a tuning variant next to the default library (development only)."""
-    lib = out or LIB
-    if not force and not defines and not needs_build():
+def build(force=False, verbose=False):
+    """Compile every translation unit for sm_90a and link the shared library. Returns the library path."""
+    if not force and not needs_build():
         return LIB
     os.makedirs(LIB_DIR, exist_ok=True)
-    obj_dir = os.path.join(HERE, "build" + ("_" + "_".join(defines).replace("=", "") if defines else ""))
+    obj_dir = os.path.join(HERE, "build")
     os.makedirs(obj_dir, exist_ok=True)
     nvcc = _nvcc()
     procs = []
     for src in SOURCES:
         obj = os.path.join(obj_dir, os.path.splitext(src)[0] + ".o")
-        cmd = [nvcc, *NVCC_FLAGS, *["-D" + d for d in defines], "-x", "cu", "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc, *NVCC_FLAGS, "-x", "cu", "-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((src, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     objs = []
     for src, obj, p in procs:
@@ -55,14 +53,10 @@ def build(force=False, verbose=False, defines=(), out=None):
         if verbose:
             sys.stderr.write(out)
         objs.append(obj)
-    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", lib, *objs, "-lcudart", "-ldl"]
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB, *objs, "-lcudart", "-ldl"]
     subprocess.check_call(cmd)
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":
-    defs = tuple(a[2:] for a in sys.argv if a.startswith("-D"))
-    outs = [a[6:] for a in sys.argv if a.startswith("--out=")]
-    if "--out" in sys.argv:
-        outs.append(sys.argv[sys.argv.index("--out") + 1])
-    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, defines=defs, out=outs[0] if outs else None))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -960,7 +960,6 @@ struct cldn_decoder {
   DevBuf<uint8_t> d_in, d_out;
   DevBuf<uint32_t> d_chunk_tiles, d_chunk_tile_begin, d_stream_end, d_tsums, d_chunk_frame, d_tile_chunk;
   DevBuf<uint64_t> d_tstatus;
-  DevBuf<uint64_t> d_trace;
   DevBuf<uint32_t> d_counter, d_redo;
   DevBuf<uint8_t> d_side;         // side mode: section values decoded ahead of the regular stream (DecLaunch::side)
   DevBuf<uint64_t> d_chunk_desc;  // chunk-sequential kernel: self-validating chunk descriptors (see walk_frame_publish)
@@ -1081,7 +1080,6 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
   CUDA_TRY(cudaMemcpyAsync(d->d_frames.p, hf, n_frames * sizeof(DecFrame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_frames.commit(hf_slot, d->stream)) return rc;
   DecLaunch L{};
-  L.par_runs = unmeasured_kernels_enabled() ? 1u : 0u;
   L.frames = d->d_frames.p;
   L.n_frames = static_cast<uint32_t>(n_frames);
   L.n_chunks_total = static_cast<uint32_t>(chunks);
@@ -1156,10 +1154,6 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
     for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
     L.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
   }
-  if (tile_parallel && getenv("CLDN_B200_TRACE")) {
-    if (int rc = d->d_trace.reserve(std::max<size_t>(L.tile_grid, static_cast<size_t>(chunks) * 80) * 8 + 8, true)) return rc;
-    L.trace = d->d_trace.p;
-  }
   d->fast_launched = L.redo_list != nullptr && decode_tiles_sequential(L.n_chunks_total) && decode_fast_enabled() && !d->plan.regular_overlap;
   if (d->fast_launched && L.chunk_desc && L.stream_end && L.chunk_counter && decode_side_plan(d->plan) && decode_fast_general_plan(d->plan) && !force_chunk) {
     // V5 sections ahead of the regular stream: compact per-chunk arrays the fast reader merges into the rows (DecLaunch::side)
@@ -1211,14 +1205,6 @@ void cldn_b200_decoder_destroy(cldn_decoder_t* d) {
 int cldn_b200_decoder_sync(cldn_decoder_t* d) {
   if (!d) { set_error("null decoder"); return CLDN_ERR_INVALID_ARGUMENT; }
   CUDA_TRY(cudaSetDevice(d->device));
-  if (const char* tp = getenv("CLDN_B200_TRACE")) {  // development aid: dump the per-tile phase timestamps
-    if (d->d_trace.p) {
-      cudaStreamSynchronize(d->stream);
-      std::vector<uint64_t> h(d->d_trace.cap);
-      cudaMemcpy(h.data(), d->d_trace.p, h.size() * 8, cudaMemcpyDeviceToHost);
-      if (FILE* f = fopen(tp, "wb")) { fwrite(h.data(), 8, h.size(), f); fclose(f); }
-    }
-  }
   return check_device_error(d->stream, d->d_err.p, d->h_err.p);
 }
 

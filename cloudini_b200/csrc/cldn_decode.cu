@@ -468,16 +468,15 @@ struct RunBatch {
   uint32_t n;
   uint32_t pos;       // parse position (bytes into the section) after this batch
   uint32_t runs_left;
-  uint32_t failed;
   unsigned long long prev;  // DeltaRle: running value in front of the next batch
 };
 
 // ---- parallel parse of a run table (Rle: raw value + uvarint length, DeltaRle: varint delta + uvarint length) -----------
-// The table is a chain of variable-length records, so the reference (and the first version of this reader) walks it
-// with one dependent parse per run. Here the next kRunPar * 20 bytes are staged in shared memory, every byte position
-// computes where the following record would start IF a record started there (one or two terminator bits, plus the raw
-// bytes of an Rle value), ONE thread follows that table from the batch's first byte (one shared-memory load per run) and
-// then every thread decodes one run with the careful readers; run starts and DeltaRle values come from two CTA scans.
+// The table is a chain of variable-length records, so the reference walks it with one dependent parse per run. Here the
+// next kRunPar * 20 bytes are staged in shared memory, every byte position computes where the following record would
+// start IF a record started there (one or two terminator bits, plus the raw bytes of an Rle value), ONE thread follows
+// that table from the batch's first byte (one shared-memory load per run) and then every thread decodes one run with
+// the careful readers; run starts and DeltaRle values come from two CTA scans.
 constexpr uint32_t kRunPar = kThreads;        // runs per iteration (one per thread)
 constexpr uint32_t kRunRecMax = 20;           // a record is at most 10 + 10 bytes (8 + 10 for Rle)
 constexpr uint32_t kRunStage = 5632;          // >= kRunPar * kRunRecMax, multiple of 32
@@ -517,7 +516,7 @@ template <int KT>
 __device__ uint32_t decode_section(const uint8_t* __restrict__ src, uint32_t avail, uint32_t n_points,
                                    const SectionField& sf, uint8_t* __restrict__ out, uint32_t step, DecShared& sh,
                                    uint8_t* tile_bytes, uint8_t* vals_raw, uint32_t* nanbits, RunBatch& rb,
-                                   DecSlot* sec_slot, uint32_t* err, bool par_runs) {
+                                   DecSlot* sec_slot, uint32_t* err) {
   if (avail < 1) {
     if (threadIdx.x == 0) report_error(err, DEV_ERR_BAD_MODE);  // "missing mode byte"
     return 0xFFFFFFFFu;
@@ -592,7 +591,7 @@ __device__ uint32_t decode_section(const uint8_t* __restrict__ src, uint32_t ava
     }
     return static_cast<uint32_t>(3ull + pal_bytes + idx_bytes);
   }
-  // Rle (2) / DeltaRle (3): a run table is parsed sequentially in batches, then expanded by all threads.
+  // Rle (2) / DeltaRle (3): a run table is parsed in batches of kRunPar records, then expanded by all threads.
   if (avail < 5) {
     if (threadIdx.x == 0) report_error(err, DEV_ERR_TRUNCATED);
     return 0xFFFFFFFFu;
@@ -602,7 +601,6 @@ __device__ uint32_t decode_section(const uint8_t* __restrict__ src, uint32_t ava
     rb.runs_left = load_u32(src + 1);
     rb.pos = 5;
     rb.start[0] = 0;
-    rb.failed = 0;
     rb.value[0] = 0;
   }
   __syncthreads();
@@ -615,63 +613,60 @@ __device__ uint32_t decode_section(const uint8_t* __restrict__ src, uint32_t ava
   uint32_t* hmask = reinterpret_cast<uint32_t*>(nx);                             // once the records are parsed: run-start marks of the
   uint32_t* hpre = hmask + kChunkPoints / 32;                                    //   batch's points + their word-prefix counts
   static_assert(2 * (kChunkPoints / 32) * 4 <= kRunStage * 2, "marks and prefix counts alias the next-record table");
-  unsigned long long prev = 0;     // DeltaRle running value of the sequential parser (thread 0 only)
   while (true) {
-    if (par_runs) {
-      const uint32_t pos = rb.pos;
-      const uint32_t want = rb.runs_left < kRunPar ? rb.runs_left : kRunPar;
-      const uint32_t rest = avail - pos;
-      const uint32_t S = rest < kRunStage ? rest : kRunStage;
-      const bool more_behind = rest > kRunStage;
-      for (uint32_t i = threadIdx.x; i < kRunStage + 32; i += blockDim.x) sb[i] = i < S ? src[pos + i] : 0x80u;
-      __syncthreads();
-      for (uint32_t w = threadIdx.x; w < kRunStage / 32 + 4; w += blockDim.x) {
-        uint32_t m = 0;
-        if (w * 32u < S) {
-  #pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint32_t t = ~*reinterpret_cast<const uint32_t*>(sb + w * 32u + 4 * k) & 0x80808080u;
-            m |= (((t >> 7) & 1u) | ((t >> 14) & 2u) | ((t >> 21) & 4u) | ((t >> 28) & 8u)) << (4 * k);
-          }
+    const uint32_t pos = rb.pos;
+    const uint32_t want = rb.runs_left < kRunPar ? rb.runs_left : kRunPar;
+    const uint32_t rest = avail - pos;
+    const uint32_t S = rest < kRunStage ? rest : kRunStage;
+    const bool more_behind = rest > kRunStage;
+    for (uint32_t i = threadIdx.x; i < kRunStage + 32; i += blockDim.x) sb[i] = i < S ? src[pos + i] : 0x80u;
+    __syncthreads();
+    for (uint32_t w = threadIdx.x; w < kRunStage / 32 + 4; w += blockDim.x) {
+      uint32_t m = 0;
+      if (w * 32u < S) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const uint32_t t = ~*reinterpret_cast<const uint32_t*>(sb + w * 32u + 4 * k) & 0x80808080u;
+          m |= (((t >> 7) & 1u) | ((t >> 14) & 2u) | ((t >> 21) & 4u) | ((t >> 28) & 8u)) << (4 * k);
         }
-        tb[w] = m;  // bytes behind S read as 0x80: no terminator there
+      }
+      tb[w] = m;  // bytes behind S read as 0x80: no terminator there
+    }
+    __syncthreads();
+    if (mode == 3) {
+      // a DeltaRle record is two varints: record r ends at terminator 2 r + 1 of the staged bytes. Word-prefix counts
+      // of the terminator bits (one CTA scan) rank every terminator; the odd-ranked ones name the next record's start.
+      uint32_t* tpre = reinterpret_cast<uint32_t*>(nx);                 // [kRunStage / 32 + 4] terminators in front of word w
+      const uint32_t nw = kRunStage / 32 + 4;
+      uint32_t terms_total;
+      {
+        const uint32_t w = threadIdx.x;
+        const uint32_t c = w < nw ? __popc(tb[w]) : 0u;
+        static_assert(kRunStage / 32 + 4 <= kThreads, "one terminator word per thread");
+        const uint32_t before = block_exclusive_scan_n<kThreads>(c, sh.scan, &terms_total);
+        if (w < nw) tpre[w] = before;
       }
       __syncthreads();
-      if (mode == 3) {
-        // a DeltaRle record is two varints: record r ends at terminator 2 r + 1 of the staged bytes. Word-prefix counts
-        // of the terminator bits (one CTA scan) rank every terminator; the odd-ranked ones name the next record's start.
-        uint32_t* tpre = reinterpret_cast<uint32_t*>(nx);                 // [kRunStage / 32 + 4] terminators in front of word w
-        const uint32_t nw = kRunStage / 32 + 4;
-        uint32_t terms_total;
-        {
-          const uint32_t w = threadIdx.x;
-          const uint32_t c = w < nw ? __popc(tb[w]) : 0u;
-          static_assert(kRunStage / 32 + 4 <= kThreads, "one terminator word per thread");
-          const uint32_t before = block_exclusive_scan_n<kThreads>(c, sh.scan, &terms_total);
-          if (w < nw) tpre[w] = before;
+      const uint32_t complete = terms_total >> 1;                        // records that end inside the staged bytes
+      // records taken this batch; a table that ends (or is damaged) inside the staged bytes hands its first incomplete
+      // record to the careful readers below, which say what is wrong with it
+      uint32_t n = complete < want ? complete : want;
+      if (n < want && (!more_behind || n == 0u)) n += 1u;
+      for (uint32_t b = threadIdx.x; b < S; b += blockDim.x) {
+        const uint32_t w = b >> 5, k = b & 31u;
+        const uint32_t word = tb[w];
+        if ((word >> k) & 1u) {
+          const uint32_t rank = tpre[w] + __popc(word & ((1u << k) - 1u));
+          if ((rank & 1u) && (rank >> 1) + 1u <= n) rs[(rank >> 1) + 1u] = static_cast<uint16_t>(b + 1u);
         }
-        __syncthreads();
-        const uint32_t complete = terms_total >> 1;                        // records that end inside the staged bytes
-        // records taken this batch; a table that ends (or is damaged) inside the staged bytes hands its first incomplete
-        // record to the careful readers below, which say what is wrong with it
-        uint32_t n = complete < want ? complete : want;
-        if (n < want && (!more_behind || n == 0u)) n += 1u;
-        for (uint32_t b = threadIdx.x; b < S; b += blockDim.x) {
-          const uint32_t w = b >> 5, k = b & 31u;
-          const uint32_t word = tb[w];
-          if ((word >> k) & 1u) {
-            const uint32_t rank = tpre[w] + __popc(word & ((1u << k) - 1u));
-            if ((rank & 1u) && (rank >> 1) + 1u <= n) rs[(rank >> 1) + 1u] = static_cast<uint16_t>(b + 1u);
-          }
-        }
-        if (threadIdx.x == 0) {
-          rs[0] = 0;
-          if (n > complete) rs[n] = static_cast<uint16_t>(kRunNone);
-          rb.n = n;
-          rb.failed = 0;
-        }
-        __syncthreads();
-      } else {
+      }
+      if (threadIdx.x == 0) {
+        rs[0] = 0;
+        if (n > complete) rs[n] = static_cast<uint16_t>(kRunNone);
+        rb.n = n;
+      }
+      __syncthreads();
+    } else {
       for (uint32_t b = threadIdx.x; b < S; b += blockDim.x) {
         uint32_t p = b + bpv;
         if (p > S) p = kRunNone;
@@ -689,148 +684,96 @@ __device__ uint32_t decode_section(const uint8_t* __restrict__ src, uint32_t ava
         }
         rs[n] = static_cast<uint16_t>(p);
         rb.n = n;
-        rb.failed = 0;
       }
       __syncthreads();
+    }
+    {
+      const uint32_t n = rb.n;
+      const uint32_t r = threadIdx.x;
+      bool bad = false;
+      unsigned long long run_len = 0, raw = 0;
+      long long diff = 0;
+      uint32_t q = 0;
+      if (r < n) {
+        q = rs[r];
+        if (mode == 2) {
+          if (rest - q < bpv) { report_error(err, DEV_ERR_RLE); bad = true; }  // "truncated RLE value"
+          else { raw = load_raw_bits(sb + q, bpv); q += bpv; }
+        } else {
+          const uint32_t lim = (rest - q) < (S - q) ? (rest - q) : (S - q);
+          const uint32_t c = read_varint(sb + q, lim, &diff, err);
+          if (!c) bad = true;
+          q += c;
+        }
+        if (!bad) {
+          const uint32_t lim = (rest - q) < (S - q) ? (rest - q) : (S - q);
+          const uint32_t c2 = read_uvarint(sb + q, lim, &run_len, err);
+          if (!c2) bad = true;
+          q += c2;
+        }
       }
+      if (__syncthreads_or(bad ? 1 : 0)) return 0xFFFFFFFFu;
+      // run starts: exclusive sum of the lengths (64-bit: a forged length must not wrap)
+      unsigned long long len_total, prod_total;
+      const unsigned long long before = block_exclusive_sum_u64(r < n ? run_len : 0ull, sh.seg_sum, &len_total);
+      const unsigned long long oi = static_cast<unsigned long long>(out_index) + before;
+      if (r < n && (oi > n_points || run_len > static_cast<unsigned long long>(n_points) - oi)) {  // "run exceeds point count"
+        report_error(err, DEV_ERR_RLE);
+        bad = true;
+      }
+      // DeltaRle: the value in front of run r is prev + sum over earlier runs of diff * length (wrapping like the reference)
+      const unsigned long long prod = (r < n && mode == 3) ? static_cast<unsigned long long>(diff) * run_len : 0ull;
+      const unsigned long long pbefore = block_exclusive_sum_u64(prod, sh.seg_sum, &prod_total);
+      if (__syncthreads_or(bad ? 1 : 0)) return 0xFFFFFFFFu;
+      // Which run does point i belong to? One bit per point of the batch marks the run starts; a point's run is the
+      // number of marks up to it (word-prefix counts + one popc) -- two shared-memory loads instead of a binary search
+      // over the starts (8 dependent loads; 45 % of the kernel's instructions on a 64-ring `ring` field). Empty runs
+      // set no mark and get no slot.
+      const bool ne = r < n && run_len > 0ull;
+      uint32_t ne_total;
+      const uint32_t slot = block_exclusive_scan_n<kThreads>(ne ? 1u : 0u, sh.scan, &ne_total);
+      const uint32_t batch_pts = static_cast<uint32_t>(len_total);       // validated above: <= n_points - out_index
+      const uint32_t mw = (batch_pts + 31u) / 32u;
+      for (uint32_t w = threadIdx.x; w < mw; w += blockDim.x) hmask[w] = 0u;
+      __syncthreads();
+      if (ne) {
+        const uint32_t rel = static_cast<uint32_t>(oi) - out_index;
+        atomicOr(&hmask[rel >> 5], 1u << (rel & 31u));
+        rb.start[slot] = static_cast<uint32_t>(oi);
+        rb.value[slot] = mode == 2 ? raw : rb.prev + pbefore;
+        rb.diff[slot] = diff;
+      }
+      if (r + 1 == n) rb.pos = pos + q;
+      __syncthreads();  // marks complete; everybody has read rb.prev / rb.runs_left / rb.n
       {
-        const uint32_t n = rb.n;
-        const uint32_t r = threadIdx.x;
-        bool bad = false;
-        unsigned long long run_len = 0, raw = 0;
-        long long diff = 0;
-        uint32_t q = 0;
-        if (r < n) {
-          q = rs[r];
-          if (mode == 2) {
-            if (rest - q < bpv) { report_error(err, DEV_ERR_RLE); bad = true; }  // "truncated RLE value"
-            else { raw = load_raw_bits(sb + q, bpv); q += bpv; }
-          } else {
-            const uint32_t lim = (rest - q) < (S - q) ? (rest - q) : (S - q);
-            const uint32_t c = read_varint(sb + q, lim, &diff, err);
-            if (!c) bad = true;
-            q += c;
-          }
-          if (!bad) {
-            const uint32_t lim = (rest - q) < (S - q) ? (rest - q) : (S - q);
-            const uint32_t c2 = read_uvarint(sb + q, lim, &run_len, err);
-            if (!c2) bad = true;
-            q += c2;
-          }
-        }
-        if (__syncthreads_or(bad ? 1 : 0)) return 0xFFFFFFFFu;
-        // run starts: exclusive sum of the lengths (64-bit: a forged length must not wrap)
-        unsigned long long len_total, prod_total;
-        const unsigned long long before = block_exclusive_sum_u64(r < n ? run_len : 0ull, sh.seg_sum, &len_total);
-        const unsigned long long oi = static_cast<unsigned long long>(out_index) + before;
-        if (r < n && (oi > n_points || run_len > static_cast<unsigned long long>(n_points) - oi)) {  // "run exceeds point count"
-          report_error(err, DEV_ERR_RLE);
-          bad = true;
-        }
-        // DeltaRle: the value in front of run r is prev + sum over earlier runs of diff * length (wrapping like the reference)
-        const unsigned long long prod = (r < n && mode == 3) ? static_cast<unsigned long long>(diff) * run_len : 0ull;
-        const unsigned long long pbefore = block_exclusive_sum_u64(prod, sh.seg_sum, &prod_total);
-        if (__syncthreads_or(bad ? 1 : 0)) return 0xFFFFFFFFu;
-        // Which run does point i belong to? One bit per point of the batch marks the run starts; a point's run is the
-        // number of marks up to it (word-prefix counts + one popc) -- two shared-memory loads instead of a binary search
-        // over the starts (8 dependent loads; 45 % of the kernel's instructions on a 64-ring `ring` field). Empty runs
-        // set no mark and get no slot.
-        const bool ne = r < n && run_len > 0ull;
-        uint32_t ne_total;
-        const uint32_t slot = block_exclusive_scan_n<kThreads>(ne ? 1u : 0u, sh.scan, &ne_total);
-        const uint32_t batch_pts = static_cast<uint32_t>(len_total);       // validated above: <= n_points - out_index
-        const uint32_t mw = (batch_pts + 31u) / 32u;
-        for (uint32_t w = threadIdx.x; w < mw; w += blockDim.x) hmask[w] = 0u;
-        __syncthreads();
-        if (ne) {
-          const uint32_t rel = static_cast<uint32_t>(oi) - out_index;
-          atomicOr(&hmask[rel >> 5], 1u << (rel & 31u));
-          rb.start[slot] = static_cast<uint32_t>(oi);
-          rb.value[slot] = mode == 2 ? raw : rb.prev + pbefore;
-          rb.diff[slot] = diff;
-        }
-        if (r + 1 == n) rb.pos = pos + q;
-        __syncthreads();  // marks complete; everybody has read rb.prev / rb.runs_left / rb.n
-        {
-          constexpr uint32_t kPer = kChunkPoints / 32 / kThreads;           // mask words per thread
-          const uint32_t w0 = kPer * threadIdx.x;
-          uint32_t c = 0;
+        constexpr uint32_t kPer = kChunkPoints / 32 / kThreads;           // mask words per thread
+        const uint32_t w0 = kPer * threadIdx.x;
+        uint32_t c = 0;
 #pragma unroll
-          for (uint32_t k = 0; k < kPer; ++k) c += (w0 + k < mw) ? __popc(hmask[w0 + k]) : 0u;
-          uint32_t marks;
-          uint32_t before = block_exclusive_scan_n<kThreads>(c, sh.scan, &marks);
+        for (uint32_t k = 0; k < kPer; ++k) c += (w0 + k < mw) ? __popc(hmask[w0 + k]) : 0u;
+        uint32_t marks;
+        uint32_t before = block_exclusive_scan_n<kThreads>(c, sh.scan, &marks);
 #pragma unroll
-          for (uint32_t k = 0; k < kPer; ++k) {
-            if (w0 + k < mw) { hpre[w0 + k] = before; before += __popc(hmask[w0 + k]); }
-          }
-        }
-        if (threadIdx.x == 0) {
-          rb.start[ne_total] = out_index + batch_pts;
-          rb.n = ne_total;
-          rb.prev += prod_total;
-          rb.runs_left -= n;
+        for (uint32_t k = 0; k < kPer; ++k) {
+          if (w0 + k < mw) { hpre[w0 + k] = before; before += __popc(hmask[w0 + k]); }
         }
       }
-    } else {  // hardware-verified sequential parse: thread 0 walks up to kRunBatch records
       if (threadIdx.x == 0) {
-        uint32_t n = 0, pos = rb.pos, oi = out_index;
-        while (n < kRunBatch && rb.runs_left > 0) {
-          unsigned long long run_len = 0;
-          if (mode == 2) {
-            if (avail - pos < bpv) { report_error(err, DEV_ERR_RLE); rb.failed = 1; break; }  // "truncated RLE value"
-            rb.value[n] = load_raw_bits(src + pos, bpv);
-            pos += bpv;
-          } else {
-            long long diff;
-            const uint32_t c = read_varint(src + pos, avail - pos, &diff, err);
-            if (!c) { rb.failed = 1; break; }
-            pos += c;
-            rb.diff[n] = diff;
-            rb.value[n] = prev;
-          }
-          const uint32_t c2 = read_uvarint(src + pos, avail - pos, &run_len, err);
-          if (!c2) { rb.failed = 1; break; }
-          pos += c2;
-          if (run_len > static_cast<unsigned long long>(n_points - oi)) {  // "run exceeds point count"
-            report_error(err, DEV_ERR_RLE);
-            rb.failed = 1;
-            break;
-          }
-          if (mode == 3) prev += static_cast<unsigned long long>(rb.diff[n]) * run_len;
-          rb.start[n] = oi;
-          oi += static_cast<uint32_t>(run_len);
-          --rb.runs_left;
-          ++n;
-        }
-        rb.start[n] = oi;
-        rb.n = n;
-        rb.pos = pos;
+        rb.start[ne_total] = out_index + batch_pts;
+        rb.n = ne_total;
+        rb.prev += prod_total;
+        rb.runs_left -= n;
       }
     }
     __syncthreads();
-    if (rb.failed) return 0xFFFFFFFFu;
     const uint32_t n = rb.n;
     const uint32_t lo_pt = out_index, hi_pt = rb.start[n];
-    if (par_runs) {
-      for (uint32_t i = lo_pt + threadIdx.x; i < hi_pt; i += blockDim.x) {
-        const uint32_t rel = i - lo_pt, w = rel >> 5;
-        const uint32_t run = hpre[w] + __popc(hmask[w] & (0xFFFFFFFFu >> (31u - (rel & 31u)))) - 1u;
-        unsigned long long v = rb.value[run];
-        if (mode == 3) v += static_cast<unsigned long long>(rb.diff[run]) * static_cast<unsigned long long>(i - rb.start[run] + 1);
-        if (sf.offset != CLDN_SKIP_STORE_OFFSET) store_low_bytes(out + static_cast<size_t>(i) * step + sf.offset, v, bpv);
-      }
-    } else {
     for (uint32_t i = lo_pt + threadIdx.x; i < hi_pt; i += blockDim.x) {
-      // last run with start <= i (empty runs share their start with the next run and are skipped by the search)
-      uint32_t lo = 0, hi = n - 1;
-      while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (rb.start[mid] <= i) lo = mid; else hi = mid - 1;
-      }
-      unsigned long long v = rb.value[lo];
-      if (mode == 3) v += static_cast<unsigned long long>(rb.diff[lo]) * static_cast<unsigned long long>(i - rb.start[lo] + 1);
+      const uint32_t rel = i - lo_pt, w = rel >> 5;
+      const uint32_t run = hpre[w] + __popc(hmask[w] & (0xFFFFFFFFu >> (31u - (rel & 31u)))) - 1u;
+      unsigned long long v = rb.value[run];
+      if (mode == 3) v += static_cast<unsigned long long>(rb.diff[run]) * static_cast<unsigned long long>(i - rb.start[run] + 1);
       if (sf.offset != CLDN_SKIP_STORE_OFFSET) store_low_bytes(out + static_cast<size_t>(i) * step + sf.offset, v, bpv);
-    }
     }
     out_index = hi_pt;
     const uint32_t left = rb.runs_left;
@@ -925,7 +868,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const DecLaunch
       if (sf.offset != CLDN_SKIP_STORE_OFFSET) sf.offset = 0;
     }
     const uint32_t used = decode_section<KT>(body + pos, body_bytes - pos, n_points, sf, dst, dstep,
-                                             sh, tile_bytes, vals_raw, nanbits, rb, &s_slots[kMaxOps], err, L.par_runs != 0);
+                                             sh, tile_bytes, vals_raw, nanbits, rb, &s_slots[kMaxOps], err);
     if (used == 0xFFFFFFFFu) {
       if (side && threadIdx.x == 0) L.stream_end[gc] = 0xFFFFFFFFu;
       return;
@@ -1271,42 +1214,26 @@ __global__ void __launch_bounds__(kThreads) decode_mixed_kernel(const DecLaunch 
     }
     __syncthreads();
     // ---- 3. pointer doubling: round k appends boundaries 2^k .. 2^(k+1)-1 and squares the jump table ----
-    //         (or, L.mix_chase: one thread follows next() through the tile — 1/10 of the work, one dependent
-    //         shared-memory load per point; which one wins depends on how many chunks are in flight)
     uint16_t* jt = jump0;
     uint16_t* jn = jump1;
     uint32_t exit_pos = kMixNone;
-    if (L.mix_chase) {
-      if (threadIdx.x == 0) {
-        uint32_t i = 0, p = mis;
-        while (p < kMixTile && i < kMixTile) {
-          starts[i++] = static_cast<uint16_t>(p);
-          p = jump0[p];
+    for (uint32_t step = 1; step < kMixTile; step <<= 1) {  // a tile holds at most kMixTile boundaries (one per byte)
+      int grew = 0;
+      for (uint32_t i = threadIdx.x; i < step; i += blockDim.x) {
+        const uint32_t b = starts[i];
+        if (b != kMixNone) {
+          const uint32_t t = jt[b];
+          if (t < kMixTile) { starts[i + step] = static_cast<uint16_t>(t); grew = 1; }
         }
-        ms.n_found = i;
-        jump1[0] = static_cast<uint16_t>(p);  // the exit position travels through shared memory
+      }
+      if (!__syncthreads_or(grew)) { exit_pos = jt[mis]; break; }  // no boundary beyond 2^k: jt[entry] already left the tile
+      for (uint32_t b = threadIdx.x; b < kMixTile; b += blockDim.x) {
+        const uint32_t t = jt[b];
+        jn[b] = (t < kMixTile) ? jt[t] : static_cast<uint16_t>(t);
       }
       __syncthreads();
-      exit_pos = jump1[0];
-    } else {
-      for (uint32_t step = 1; step < kMixTile; step <<= 1) {  // a tile holds at most kMixTile boundaries (one per byte)
-        int grew = 0;
-        for (uint32_t i = threadIdx.x; i < step; i += blockDim.x) {
-          const uint32_t b = starts[i];
-          if (b != kMixNone) {
-            const uint32_t t = jt[b];
-            if (t < kMixTile) { starts[i + step] = static_cast<uint16_t>(t); grew = 1; }
-          }
-        }
-        if (!__syncthreads_or(grew)) { exit_pos = jt[mis]; break; }  // no boundary beyond 2^k: jt[entry] already left the tile
-        for (uint32_t b = threadIdx.x; b < kMixTile; b += blockDim.x) {
-          const uint32_t t = jt[b];
-          jn[b] = (t < kMixTile) ? jt[t] : static_cast<uint16_t>(t);
-        }
-        __syncthreads();
-        uint16_t* sw = jt; jt = jn; jn = sw;
-        exit_pos = jt[mis];
-      }
+      uint16_t* sw = jt; jt = jn; jn = sw;
+      exit_pos = jt[mis];
     }
     {  // number of boundaries = first unset entry of the list
       uint32_t mine = 0;
@@ -1410,8 +1337,8 @@ static size_t mixed_smem_bytes(const Plan& plan) {
 // point fits the look-ahead of a tile.
 static bool mixed_plan_ok(const Plan& plan) {
   if (plan.n_gorilla != 0 || plan.max_point_bytes > kMixLook || plan.n_ops == 0) return false;
-  const char* e = getenv("CLDN_B200_MIXED_DECODE");  // "par" / "chase" / "seq": explicit choice
-  return e ? e[0] != 's' : unmeasured_kernels_enabled();
+  const char* e = getenv("CLDN_B200_MIXED_DECODE");  // "par" / "seq": explicit choice
+  return !(e && e[0] == 's');
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1771,7 +1698,7 @@ static size_t gorilla_smem_bytes(const Plan& plan) {
 static bool gorilla_plan_ok(const Plan& plan) {
   if (plan.n_gorilla != 1 || plan.max_point_bytes > kMixLook) return false;
   const char* e = getenv("CLDN_B200_MIXED_DECODE");
-  return e ? e[0] != 's' : unmeasured_kernels_enabled();
+  return !(e && e[0] == 's');
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1928,10 +1855,7 @@ int launch_decode(const Plan& plan, const DecLaunch& L, cudaStream_t stream) {
       if (mixed_plan_ok(plan)) {
         const size_t msmem = mixed_smem_bytes(plan);
         if (raise_smem_limit(decode_mixed_kernel, msmem) != cudaSuccess) return -1;
-        DecLaunch M = L;
-        const char* mm = getenv("CLDN_B200_MIXED_DECODE");  // "chase": development override (see the kernel)
-        M.mix_chase = (mm && mm[0] == 'c') ? 1u : 0u;
-        decode_mixed_kernel<<<L.n_chunks_total, kThreads, msmem, stream>>>(M);
+        decode_mixed_kernel<<<L.n_chunks_total, kThreads, msmem, stream>>>(L);
       } else if (gorilla_plan_ok(plan)) {
         const size_t gsmem = gorilla_smem_bytes(plan);
         if (raise_smem_limit(decode_gorilla_kernel, gsmem) != cudaSuccess) return -1;

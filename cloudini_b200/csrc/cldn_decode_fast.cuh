@@ -30,36 +30,19 @@ constexpr int kFW = kFT / 32;                // warps
 // Values 0 .. n_floatn-1 of a point are the FloatN group (int32 arithmetic, wrapping like the reference's Vector4i); the
 // rest are scalar lossy FLOAT32 fields, which the reference accumulates in int64 (field_decoder.hpp:331-353): the fast
 // reader keeps 64-bit bases for them and hands the chunk to the careful kernel if a value leaves the int32 range.
-#ifndef CLDN_FAST_DEC_DIRECT
-#define CLDN_FAST_DEC_DIRECT 0   // 1 = dense XYZI stores its floats straight from registers and requests the next window early: measured slower (32 lanes x 16 B at a 128-byte stride per store instruction)
-#endif
-#ifndef CLDN_FAST_DEC_SPLIT
-#define CLDN_FAST_DEC_SPLIT 0   // 1 = <= 4 values per point stage their floats in their own 8 KB (two half passes of 64-byte pieces), request the next
-                                //     window behind the parse barrier and drop the end-of-tile barrier: measured slower
-#endif
-#ifndef CLDN_FAST_DEC_CPASYNC
-#define CLDN_FAST_DEC_CPASYNC 1   // window staging by cp.async, measured faster than plain loads + stores (0)
-#endif
-#ifndef CLDN_FAST_DEC_ROLLING
-#define CLDN_FAST_DEC_ROLLING 1
-#endif
-#ifndef CLDN_FAST_DEC_MINB
-#define CLDN_FAST_DEC_MINB 7   // resident CTAs per SM the register allocation aims at (8 spills; 6 loses more than it gains: profiles/r2_variants.txt)
-#endif
+constexpr int kFastDecMinBlocks = 7;   // resident CTAs per SM the register allocation aims at (8 spills; 6 loses more than it gains)
 struct FastDecParams {
   float mul[6];
   uint32_t off[6];
   uint32_t n_floatn;
-  uint32_t rows;   // 1: the regular fields and the V5 section fields together cover every byte of a point, whole rows may be written;
-                   // 2: every field lies inside the point but some bytes belong to none (rows leave word by word, padding masked); 0: neither
-  uint64_t cover;  // rows == 2: bit b set <=> byte b of a point belongs to a field
+  uint32_t rows;   // 1: the regular fields and the V5 section fields together cover every byte of a point, whole rows may be written
   // side mode (SIDE instantiations): the V5 section fields whose values wait in DecLaunch::side
   uint32_t n_side;
   uint32_t side_offset[kMaxSideFields];   // byte offset inside a point (CLDN_SKIP_STORE_OFFSET: decoded, not stored)
   uint32_t side_bpv[kMaxSideFields];
 };
 constexpr int kFUnit = 16;                   // bytes per unit: a thread's slice of the window is `nu` units (nu odd: the
-constexpr int kFMaxUnits = CLDN_FAST_DEC_SPLIT ? 9 : 11;   //   16-byte reads of a warp are then conflict-free at any count)
+constexpr int kFMaxUnits = 11;                //   16-byte reads of a warp are then conflict-free at any count)
 constexpr int kFLead = 16;                   // bytes in front of the window (never read as data; keeps indices > 0)
 constexpr int kFWinBytes = kFMaxUnits * kFT * kFUnit;   // 22528
 constexpr int kFWinAlloc = kFLead + kFWinBytes + 160;   // a thread's reader may run 32 values x 4 bytes (garbage behind its last real
@@ -74,8 +57,6 @@ constexpr int kFSideMaxUnits = 9;
 constexpr int kFSideOff = (kFLead + kFSideMaxUnits * kFT * kFUnit + 160 + 15) & ~15;   // 18608
 constexpr int kFSideBytes = 8192;                        // sum over the section fields of tile points * bpv fits here (decode_side_plan)
 static_assert(kFT * 8 * 16 <= kFSideOff, "the float staging aliases the window, not the section values");
-constexpr int kFOut2Off = (kFWinAlloc + 15) & ~15;      // split staging (SPLIT): 4 slots per lane, private to each warp, behind the window
-constexpr int kFOut2Bytes = kFT * 4 * 16;               // 8 KB
 
 struct FastShared {
   uint32_t wcnt[kFW];                 // terminators per warp
@@ -144,11 +125,10 @@ __device__ __forceinline__ uint64_t load_side_value(const uint8_t* p, uint32_t b
 // SIDE: the chunk's V5 sections were decoded ahead of this kernel into DecLaunch::side (stream_end_kernel found where
 // they start); their values are merged into the rows as they are written, so every output sector is written by ONE pass.
 template <int K, int FP, bool MIXED, bool ROWS, int NF, bool SIDE>   // NF: lanes of the leading FloatN group (K when !MIXED)
-__global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_kernel(const DecLaunch L, const FastDecParams Q) {
+__global__ void __launch_bounds__(kFT, kFastDecMinBlocks) decode_floatn_fast_kernel(const DecLaunch L, const FastDecParams Q) {
   constexpr int kFP = FP;
   constexpr int kFTilePts = kFT * FP;
   constexpr int kSlots = K <= 4 ? 1 : 2;                     // 16-byte staging slots per point
-  constexpr bool kSplit = CLDN_FAST_DEC_SPLIT && CLDN_FAST_DEC_CPASYNC && K <= 4 && FP == 8 && !ROWS && !SIDE;
   constexpr int kMaxU = SIDE ? (kFSideMaxUnits < kFMaxUnits ? kFSideMaxUnits : kFMaxUnits) : kFMaxUnits;   // window units per thread
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   __shared__ FastShared sh;
@@ -231,16 +211,12 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
     // shared memory and writes them with 16-byte stores. Per-field 4-byte stores of 32 lanes touch one 32-byte sector
     // per lane and field (XYZIRT, step 22: 16 sectors per store instruction measured, 5x the row bytes through L2).
     // A warp's staging holds 4 KB: layouts whose 32 * FP rows need more go out in 2, 4 or 8 passes of contiguous rows (the
-    // owner lanes of a pass fill it, everybody copies it out). Q.rows == 2: some bytes of a point belong to no field
-    // (padding) and must keep what the caller's buffer holds: the rows leave word by word, 32 consecutive words per store
-    // instruction, with the padding words switched off -- every sector is written once, where per-field stores write it
-    // once per field (measured on C3, step 32: the per-field reader is bound by L2 sector writes, 5 per point). Fetching
-    // the old rows to write whole ones was measured too, slower on C3 (a second 32 B per point from DRAM, and every
-    // pass of a warp waits for them).
+    // owner lanes of a pass fill it, everybody copies it out). A layout with padding bytes keeps per-field stores: the
+    // padding must keep what the caller's buffer holds. Fetching the old rows to write whole ones was measured, slower on
+    // C3 (a second 32 B per point from DRAM, and every pass of a warp waits for them).
     uint32_t rows_shift = 0;
     while (((step * (32u * kFP)) >> rows_shift) > 4096u && rows_shift < 3u) ++rows_shift;
     const bool rows = ROWS && !dense4 && Q.rows != 0u && ((step * (32u * kFP)) >> rows_shift) <= 4096u && (reinterpret_cast<uintptr_t>(out) & 15u) == 0u;
-    const bool rows_holes = Q.rows == 2u;
     uint32_t row_align = step;
 #pragma unroll
     for (int f = 0; f < K; ++f) row_align |= off[f];
@@ -252,13 +228,6 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
     for (int f = 0; f < K; ++f) { carry[f] = 0; if (MIXED) carry64[f] = 0; }
     uint32_t cursor = 0;                      // stream byte offset of the next tile's first value
     uint32_t est = 0;                         // bytes of the previous tile (0: none yet)
-    // Dense XYZI (one 16-byte store per point): a thread's 8 consecutive points leave straight from its registers, 16
-    // bytes each. Nothing aliases the window then, so once every thread has parsed (the any_bad barrier) the NEXT tile's
-    // window is requested with cp.async and lands while this tile is summed, converted and stored; the barrier that
-    // separated the staged copy-out from the next staging is gone.
-    const bool direct = CLDN_FAST_DEC_DIRECT && CLDN_FAST_DEC_CPASYNC && K == 4 && !MIXED && !ROWS && !SIDE && dense4;
-    bool pre = false;                         // the next tile's window has been requested ...
-    uint32_t pre_nu = 0;                      // ... with this many units per thread
     bool redo = (size == 0u);                 // an empty body cannot hold n_points > 0 points: the careful kernel reports it
     if (SIDE) redo = redo || L.stream_end[gc] == 0xFFFFFFFFu;   // no stream end / a damaged section: nothing to merge, the careful kernels decide
     for (uint32_t pt0 = 0; pt0 < n_points && !redo; pt0 += kFTilePts) {
@@ -275,7 +244,6 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
       uint32_t nu = (want + (kFT * kFUnit - 1)) / (kFT * kFUnit);
       nu = nu < 3u ? 3u : (nu | 1u);
       if (nu > kMaxU) nu = kMaxU;
-      if (pre) nu = pre_nu;
       if (SIDE) {
         // the tile's section values (whole tile: a chunk's slot holds kChunkPoints values whatever its point count) are
         // requested now and land while the window is staged and parsed
@@ -304,37 +272,16 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
         const uint32_t v_hi = room < n_vec ? static_cast<uint32_t>(room) : n_vec;
         const uint4* gv = reinterpret_cast<const uint4*>(abase) + threadIdx.x;
         uint4* sv = reinterpret_cast<uint4*>(win + kFLead) + threadIdx.x;
-        if (pre) {
-          async_wait_all();   // requested behind the previous tile's parse
-          pre = false;
-        } else if (v_lo == 0u && v_hi == n_vec) {
-#if CLDN_FAST_DEC_CPASYNC
+        if (v_lo == 0u && v_hi == n_vec) {
           // the whole window lies inside the payload (every tile but the first / last few of a frame): cp.async, global ->
-          // shared without the register round trip, every request of the thread in flight at once
+          // shared without the register round trip, every request of the thread in flight at once (measured faster than
+          // plain loads + stores)
 #pragma unroll
           for (int r = 0; r < kMaxU; ++r) {
             if (r < static_cast<int>(nu)) async_copy16(sv + r * kFT, gv + r * kFT);
           }
           async_commit();
           async_wait_all();
-#else
-          // the whole window lies inside the payload (every tile but the first / last few of a frame): plain loads, all of
-          // a thread's requests in flight before the first store
-#pragma unroll
-          for (int r0 = 0; r0 < kMaxU; r0 += 4) {   // 4 requests in flight per thread and round (16 registers)
-            if (r0 < static_cast<int>(nu)) {
-              uint4 q[4];
-#pragma unroll
-              for (int r = 0; r < 4; ++r) {
-                if (r0 + r < static_cast<int>(nu)) q[r] = __ldcs(gv + (r0 + r) * kFT);
-              }
-#pragma unroll
-              for (int r = 0; r < 4; ++r) {
-                if (r0 + r < static_cast<int>(nu)) sv[(r0 + r) * kFT] = q[r];
-              }
-            }
-          }
-#endif
         } else {
 #pragma unroll 1
           for (uint32_t r = 0; r < nu; ++r) {
@@ -434,28 +381,20 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
 #pragma unroll
         for (int f = 0; f < K; ++f) acc[f] = 0;
         const uint32_t* win32 = reinterpret_cast<const uint32_t*>(win);
-#if CLDN_FAST_DEC_ROLLING
         // rolling 64-bit window: the shared-memory loads follow the WORD index, which only ever steps by one, so the next
         // word is in a register before it is needed and no load sits on the value-to-value dependency chain
         uint32_t wi = pb >> 5;
         uint32_t lo = win32[wi], hi = win32[wi + 1], nx = win32[wi + 2u];   // (kFWinAlloc leaves room behind the window)
-#endif
 #pragma unroll
         for (int j = 0; j < kFP; ++j) {
 #pragma unroll
           for (int f = 0; f < K; ++f) {
-#if CLDN_FAST_DEC_ROLLING
             const uint32_t w = __funnelshift_r(lo, hi, pb);                    // the 4 bytes at the bit position pb
-#else
-            const uint32_t wi = pb >> 5;
-            const uint32_t w = __funnelshift_r(win32[wi], win32[wi + 1], pb);  // the 4 bytes at the bit position pb
-#endif
             const uint32_t t = ~w & 0x80808080u;                               // terminators among them
             const uint32_t msk = t ^ (t - 1u);                                 // everything up to the first one (all if none)
             uint32_t x = w & 0x7F7F7F7Fu & msk;                                // the value's payload bits
             trk = min3_u32(trk, t, x);                                         // 0 <=> no terminator in 4 bytes, or a zero value
             pb += __popc(msk);
-#if CLDN_FAST_DEC_ROLLING
             if ((pb >> 5) != wi) {                                             // a value is at most 32 bits: one word step at most
               ++wi;
               lo = hi;
@@ -467,7 +406,6 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
             // a predicated load of `hi` (5 instructions), and a mask from wi - wn with two LOP3 and an unconditional load (6):
             // both slower per 128 frames. Fewer instructions, slower: the kernel is not bound by issue slots
             // alone at this point of the loop)
-#endif
             x = x - ((x >> 1) & 0x3F803F80u);                                  // 7-bit groups -> 14-bit groups
             const uint32_t z = bitselect(0x3FFFu, x, x >> 2);                  // -> uval = zigzag + 1 (28 bits)
             // un-zigzag of z - 1: odd z -> +(z >> 1), even z -> -(z >> 1); bit 0 of z is bit 0 of the window
@@ -556,109 +494,6 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
       }
       const uint32_t ncur = sh.next_cursor;
       const uint32_t used = ncur - (kFLead + c0);
-      if (direct || kSplit) {
-        // ---- request the next tile's window (same sizing rule as the loop head, est = used): every thread has parsed, and
-        //      neither variant stages its floats inside the window ----
-        if (pt0 + kFTilePts < n_points) {
-          const uint32_t ncursor = cursor + used;
-          const uint8_t* nfirst = body + ncursor;
-          const uint32_t nc0 = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(nfirst) & 15u);
-          const uint8_t* nab = nfirst - nc0;
-          uint32_t nnu = (nc0 + used + (used >> 3) + 96u + (kFT * kFUnit - 1)) / (kFT * kFUnit);
-          nnu = nnu < 3u ? 3u : (nnu | 1u);
-          if (nnu > kMaxU) nnu = kMaxU;
-          if (ncursor < size && nab >= sh.pay_lo && (static_cast<uint64_t>(sh.pay_hi - nab) >> 4) >= nnu * kFT) {
-            const uint4* gv = reinterpret_cast<const uint4*>(nab) + threadIdx.x;
-            uint4* sv = reinterpret_cast<uint4*>(win + kFLead) + threadIdx.x;
-#pragma unroll
-            for (int r = 0; r < kMaxU; ++r) {
-              if (r < static_cast<int>(nnu)) async_copy16(sv + r * kFT, gv + r * kFT);
-            }
-            async_commit();
-            pre = true;
-            pre_nu = nnu;
-          }
-          // ... and the tile after it into L2
-          const uint32_t ahead = ncursor + used + threadIdx.x * 128u;
-          if (ahead < size && threadIdx.x * 128u < used + (used >> 2) + 256u) prefetch_l2(body + ahead);
-        }
-      }
-      if (direct) {
-        // ---- my points, 16 bytes each, straight from the registers ----
-        uint8_t* dst = out + static_cast<size_t>(pt0 + threadIdx.x * kFP) * 16u;
-#pragma unroll
-        for (int j = 0; j < kFP; ++j) {
-          uint32_t fl[4];
-#pragma unroll
-          for (int f = 0; f < 4; ++f) {
-            const int32_t v = static_cast<int32_t>(static_cast<uint32_t>(base[f < K ? f : 0]) + static_cast<uint32_t>(P[j][f < K ? f : 0]));
-            fl[f] = __float_as_uint(__fmul_rn(__int2float_rn(v), mul[f < K ? f : 0]));
-          }
-          if (static_cast<uint32_t>(j) < my_pts) __stcs(reinterpret_cast<uint4*>(dst + 16 * j), make_uint4(fl[0], fl[1], fl[2], fl[3]));
-        }
-        est = used;
-        cursor += used;
-        continue;   // no barrier: the next staging waits for its own copies, and nothing of this tile lives in shared memory
-      }
-      if (kSplit) {
-        // ---- two half passes through 4 private slots per lane: lane l stages its points 4 h .. 4 h + 3, then lanes 4 m .. 4 m + 3
-        //      store the four consecutive points of owner lane 8 i + m (64 contiguous bytes for XYZI: full sectors) ----
-        uint4* wst2 = reinterpret_cast<uint4*>(dyn_smem + kFOut2Off) + warp * (32 * 4);
-        const uint32_t wp0 = pt0 + warp * (32 * kFP);
-        const uint32_t wn = wp0 < n_points ? min(static_cast<uint32_t>(32 * kFP), n_points - wp0) : 0u;
-        const uint32_t sw = (static_cast<uint32_t>(lane) >> 1) & 3u;
-        bool wide = false;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * h + jj;
-            uint32_t fl[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-            for (int f = 0; f < K; ++f) {
-              int32_t v = static_cast<int32_t>(static_cast<uint32_t>(base[f]) + static_cast<uint32_t>(P[j][f]));
-              if (MIXED && static_cast<uint32_t>(f) >= n_floatn) {
-                const long long v64 = base64[f] + P[j][f];
-                v = static_cast<int32_t>(v64);
-                wide = wide || (v64 != static_cast<long long>(v));
-              }
-              fl[f] = __float_as_uint(__fmul_rn(__int2float_rn(v), mul[f]));
-            }
-            wst2[4 * lane + (static_cast<uint32_t>(jj) ^ sw)] = make_uint4(fl[0], fl[1], fl[2], fl[3]);
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t o = 8u * i + (static_cast<uint32_t>(lane) >> 2), jj = static_cast<uint32_t>(lane) & 3u;
-            const uint32_t q = 8u * o + 4u * h + jj;                     // point of the warp's 256
-            if (q < wn) {
-              const uint4 v = wst2[4 * o + (jj ^ ((o >> 1) & 3u))];
-              uint8_t* dst = out + static_cast<size_t>(wp0 + q) * step;
-              if (dense4) {
-                __stcs(reinterpret_cast<uint4*>(dst), v);
-              } else {
-                const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
-                if (aligned4) {
-#pragma unroll
-                  for (int f = 0; f < K; ++f) __stcs(reinterpret_cast<unsigned int*>(dst + off[f]), vv[f]);
-                } else {
-#pragma unroll
-                  for (int f = 0; f < K; ++f) {
-                    if (off[f] != CLDN_SKIP_STORE_OFFSET) store_u32(dst + off[f], vv[f]);
-                  }
-                }
-              }
-            }
-          }
-          __syncwarp();
-        }
-        est = used;
-        cursor += used;
-        if (MIXED) {
-          if (__syncthreads_or(wide ? 1 : 0)) { redo = true; break; }
-        }
-        continue;   // (plain float plans: no CTA barrier here -- the staging is private to the warp, the window is not touched)
-      }
       // the next tile's bytes are asked into L2 now (its loads are issued behind this tile's conversion and copy-out)
       if (pt0 + kFTilePts < n_points) {
         const uint32_t ahead = cursor + used + threadIdx.x * 128u;
@@ -754,31 +589,10 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
             }
           }
           __syncwarp();
-          if (rows_holes) {
-            // padded layout (step % 4 == 0): word by word, 32 consecutive words per store instruction, a word that holds padding
-            // is skipped or stored byte-wise -- the same full or partial sectors as per-field stores, once per sector
-            uint32_t r = (4u * lane) % step;             // byte offset of my word inside its row
-            const uint32_t adv = 128u % step;
-            for (uint32_t o = 4u * lane; o < total; o += 128u) {
-              const uint32_t nib = static_cast<uint32_t>(Q.cover >> r) & 0xFu;
-              const uint32_t wv = *reinterpret_cast<const uint32_t*>(wsb + o);
-              if (nib == 0xFu) {
-                __stcs(reinterpret_cast<unsigned int*>(dst + o), wv);
-              } else if (nib != 0u) {
-#pragma unroll
-                for (int b = 0; b < 4; ++b) {
-                  if ((nib >> b) & 1u) dst[o + b] = static_cast<uint8_t>(wv >> (8 * b));
-                }
-              }
-              r += adv;
-              if (r >= step) r -= step;
-            }
-          } else {
-            for (uint32_t o = 16u * lane; o + 16u <= total; o += 512u) {
-              __stcs(reinterpret_cast<uint4*>(dst + o), *reinterpret_cast<const uint4*>(wsb + o));
-            }
-            if (tail0 + lane < total) dst[tail0 + lane] = wsb[tail0 + lane];
+          for (uint32_t o = 16u * lane; o + 16u <= total; o += 512u) {
+            __stcs(reinterpret_cast<uint4*>(dst + o), *reinterpret_cast<const uint4*>(wsb + o));
           }
+          if (tail0 + lane < total) dst[tail0 + lane] = wsb[tail0 + lane];
           __syncwarp();   // the next pass refills the staging
         }
       } else if (kSlots == 1) {
@@ -880,7 +694,6 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
         __syncthreads();
       }
     }
-    if (pre) { async_wait_all(); pre = false; }   // (a tile loop left early with a window still in flight)
     if (redo) {
       if (threadIdx.x == 0) {
         L.redo_list[atomicAdd(L.chunk_counter + 3, 1u)] = gc;
@@ -902,7 +715,7 @@ __global__ void __launch_bounds__(kFT, CLDN_FAST_DEC_MINB) decode_floatn_fast_ke
 
 size_t decode_fast_smem_bytes(bool side) {
   if (side) return static_cast<size_t>(kFSideOff + kFSideBytes);
-  return static_cast<size_t>(CLDN_FAST_DEC_SPLIT ? kFOut2Off + kFOut2Bytes : kFWinAlloc);
+  return static_cast<size_t>(kFWinAlloc);
 }
 
 template <int K, int FP, bool MIXED, bool ROWS, int NF, bool SIDE>
@@ -946,7 +759,6 @@ bool decode_fast_plan(const Plan& plan, FastDecParams* Q) {
   for (int k = 0; k < kMaxSideFields; ++k) { Q->side_offset[k] = CLDN_SKIP_STORE_OFFSET; Q->side_bpv[k] = 1; }
   // rows: every byte of [0, point_step) is written by a regular field (4 bytes each here) or by a V5 section field
   Q->rows = 0;
-  Q->cover = 0;
   if (plan.point_step <= 64) {
     uint64_t covered = 0;
     bool ok = true;
@@ -960,14 +772,10 @@ bool decode_fast_plan(const Plan& plan, FastDecParams* Q) {
       covered |= ((1ull << sf.bpv) - 1ull) << sf.offset;
     }
     const uint64_t all = plan.point_step == 64 ? ~0ull : ((1ull << plan.point_step) - 1ull);
-    // 2 (padding bytes): rows assembled in shared memory, stored word by word with the padding masked -- only on request
-    // (CLDN_B200_DECODE_ROWS_HOLES=1). Measured on C3 (32 x 1M points, step 32): slower than per-field stores.
-    // The rows of a thread's 8 consecutive points lie 8 * 32 bytes apart in the staging, so every shared-memory store of
-    // the row assembly is a 32-way bank conflict (XYZIRT's 22-byte rows: 4-way), and a step of 32 needs two passes
-    const char* he = getenv("CLDN_B200_DECODE_ROWS_HOLES");
-    const bool holes = he && he[0] == '1' && (plan.point_step & 3u) == 0u;
-    Q->cover = covered;
-    if (ok) Q->rows = covered == all ? 1 : (holes ? 2 : 0);
+    // (padding bytes: per-field stores. Rows assembled in shared memory and stored word by word with the padding masked
+    // were measured on C3, 32 x 1M points, step 32: slower. The rows of a thread's 8 consecutive points lie 8 * 32 bytes
+    // apart in the staging, so every shared-memory store of the row assembly is a 32-way bank conflict.)
+    if (ok) Q->rows = covered == all ? 1 : 0;
   }
   return true;
 }

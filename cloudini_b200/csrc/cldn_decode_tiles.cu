@@ -20,17 +20,9 @@
 
 namespace cldn {
 
-#ifndef CLDN_KVEC
-#define CLDN_KVEC 2
-#endif
-constexpr int kVec = CLDN_KVEC;  // adjacent 16-byte vectors per thread
-#ifndef CLDN_DT
-#define CLDN_DT 256
-#endif
-constexpr int kDT = CLDN_DT;     // threads per decode CTA (tile = kDT * 16 * kVec stream bytes)
-#ifndef CLDN_SEQ_MINB
-#define CLDN_SEQ_MINB (CLDN_KVEC == 1 ? 4 : 3)
-#endif
+constexpr int kVec = 2;        // adjacent 16-byte vectors per thread
+constexpr int kDT = 256;       // threads per decode CTA (tile = kDT * 16 * kVec stream bytes)
+constexpr int kSeqMinBlocks = 3;   // resident CTAs per SM of the tile and chunk-sequential readers
 constexpr int kTB = kDT * 16 * kVec;  // stream bytes per tile (8192)
 constexpr int kTLook = 16;     // look-behind bytes staged in front of the tile
 constexpr uint32_t kRecWords = 8;  // look-back record: sum[4], rst, flag, pad, pad
@@ -301,12 +293,6 @@ __device__ __forceinline__ void copy_out_dense(const uint32_t* ostage, uint8_t* 
   }
 }
 
-__device__ __forceinline__ uint64_t gtimer() { uint64_t t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#ifdef CLDN_TRACE  // development builds only (tools_trace_decode.py): per-phase timestamps of every tile
-#define TRACE(slot) do { if (L.trace && threadIdx.x == 0) L.trace[static_cast<size_t>(gt) * 8 + (slot)] = gtimer(); } while (0)
-#else
-#define TRACE(slot) do { (void)gt; } while (0)
-#endif
 
 // ---- tile building blocks shared by the tile-parallel and the chunk-sequential kernel -------------------------------
 // Loads tile `t` of a chunk body into tile_bytes (with a 16-byte look-behind) and returns this thread's terminator mask.
@@ -641,7 +627,7 @@ __device__ __forceinline__ SegK<K> cta_seg_exclusive(const SegK<K>& mine, TileSh
 
 // ---- tile-parallel kernel: one CTA per 8 KB tile, two decoupled look-backs (small batches / single frames) ----------
 template <int K>
-__global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles_kernel(const DecLaunch L, float m0, float m1, float m2, float m3,
+__global__ void __launch_bounds__(kDT, kSeqMinBlocks) decode_tiles_kernel(const DecLaunch L, float m0, float m1, float m2, float m3,
                                                                    uint32_t o0, uint32_t o1, uint32_t o2, uint32_t o3) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   __shared__ TileShared sh;
@@ -652,7 +638,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
 
   const uint32_t gt = blockIdx.x;
   if (gt >= L.chunk_tile_begin[L.n_chunks_total]) return;
-  TRACE(0);
   const uint32_t gc = L.tile_chunk[gt];
   const DecFrame F = L.frames[L.chunk_frame[gc]];
   const uint32_t chunk = gc - F.chunk_begin;
@@ -675,13 +660,11 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
   const uint32_t tmask = tile_load_masks(tile_bytes, aligned, body, size, t, tile_b0);
   uint32_t VT;
   const uint32_t tile_cnt = tile_rank_starts<K>(tmask, tile_bytes, start16, sh.scan, &VT);
-  TRACE(1);
   // ---- look-back 1 (warp 0): values before this tile; overlapped with the value decoding of the other warps ----
   if (warp == 0) {
     const uint64_t ex = tile_lookback(L.tstatus, first_tile, gt, L.epoch, tile_cnt);
     if (lane == 0) sh.done = static_cast<uint32_t>(ex > 0xFFFFFFFFull ? 0xFFFFFFFFull : ex);
   }
-  TRACE(2);
   // ---- every thread decodes a run of VT consecutive values (VT a multiple of K) into registers ----
   const uint32_t v0 = threadIdx.x * VT;
   const uint32_t n_run = v0 < tile_cnt ? min(VT, tile_cnt - v0) : 0u;
@@ -689,9 +672,7 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
   unsigned long long nanm;
   uint32_t badcode, badk;
   tile_decode_run<VTMAX>(tile_bytes, n_run ? start16[threadIdx.x] : 0u, n_run, d, nanm, badcode, badk);
-  TRACE(3);
   __syncthreads();
-  TRACE(4);
   const uint32_t done = sh.done;
   // Tiles past the end of the regular stream (V5 sections / trailing bytes) are never waited on by anyone.
   if (done >= V) return;
@@ -709,7 +690,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
   const SegK<K> mine = seg_to_global<K>(run_reduce_local<K, VTMAX>(d, nanm, n_mine), phase);
   SegK<K> total;
   const SegK<K> ex = cta_seg_exclusive<K>(mine, sh, &total);
-  TRACE(5);
   // ---- look-back 2: per-field value at the tile start ----
   if (warp == 0) {
     SegK<K> carry_in = seg_identity<K>();
@@ -726,7 +706,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
     }
   }
   __syncthreads();
-  TRACE(6);
   const float mul[4] = {m0, m1, m2, m3};
   const uint32_t off[4] = {o0, o1, o2, o3};
   int32_t cur[K];
@@ -741,7 +720,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_tiles
     copy_out_dense(ostage, out, done, take);
   } else if (aligned4) run_emit_local<K, VTMAX, 1>(d, nanm, n_mine, cur, phase, out, pbase, step, mul, off);
   else run_emit_local<K, VTMAX, 0>(d, nanm, n_mine, cur, phase, out, pbase, step, mul, off);
-  TRACE(7);
 }
 
 // One thread follows the chunk prefixes of frame f (same checks and error codes as walk_chunks_kernel) and publishes
@@ -784,7 +762,7 @@ __device__ __forceinline__ void walk_frame_publish(const DecLaunch& L, uint32_t 
 // No inter-CTA communication at all: the value count and the per-field running values are carried in shared memory
 // from tile to tile; chunks are claimed from an atomic counter so that the SMs stay balanced.
 template <int K>
-__global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunks_seq_kernel(const DecLaunch L, float m0, float m1, float m2, float m3,
+__global__ void __launch_bounds__(kDT, kSeqMinBlocks) decode_chunks_seq_kernel(const DecLaunch L, float m0, float m1, float m2, float m3,
                                                                         uint32_t o0, uint32_t o1, uint32_t o2, uint32_t o3) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   __shared__ TileShared sh;
@@ -873,16 +851,12 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
     bool have_pre = false;
     uint4 pre = make_uint4(0, 0, 0, 0);
     for (uint32_t t = 0; t < n_tiles && done < V; ++t) {
-      const size_t gt = static_cast<size_t>(gc) * 80 + t;  // trace slot (development aid)
-      TRACE(0);
       const int64_t tile_b0 = static_cast<int64_t>(t) * kTB - mis;
       const uint32_t tmask = tile_load_masks(tile_bytes, aligned, body, size, t, tile_b0, have_pre, pre);
       have_pre = (t + 1 < n_tiles) && tile_vector_interior(size, tile_b0 + kTB, 0);
       if (have_pre) pre = tile_vector_fetch(aligned, t + 1, 0);
-      TRACE(1);
       uint32_t VT;
       const uint32_t tile_cnt = tile_rank_starts<K>(tmask, tile_bytes, start16, sh.scan, &VT);
-      TRACE(2);
       const uint32_t v0 = threadIdx.x * VT;
       const uint32_t take = min(tile_cnt, V - done);
       const uint32_t n_mine = v0 < take ? min(VT, take - v0) : 0u;  // my values that belong to the regular stream
@@ -898,7 +872,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
         if (badk < n_mine) report_frame_error(L, fidx, badcode);
       }
       if (!fast_ok || nanm != 0ull) local = run_reduce_local<K, VTMAX>(d, nanm, n_mine);  // sums with NaN resets
-      TRACE(3);
       if (take > 0 && done + take == V && threadIdx.x == (take - 1) / VT) {
         L.stream_end[gc] = static_cast<uint32_t>(tile_b0 + run_end_after(tile_bytes, start16[threadIdx.x], (take - 1) - v0) - kTLook);
       }
@@ -906,7 +879,6 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
       const SegK<K> mine = seg_to_global<K>(local, phase);
       SegK<K> total;
       const SegK<K> ex = cta_seg_exclusive<K>(mine, sh, &total);
-      TRACE(4);
       int32_t cur[K];
 #pragma unroll
       for (int j = 0; j < K; ++j) cur[j] = ((ex.rst >> j) & 1u) ? ex.sum[j] : wadd32(carry[j], ex.sum[j]);
@@ -915,13 +887,11 @@ __global__ void __launch_bounds__(kDT, CLDN_SEQ_MINB * (256 / kDT)) decode_chunk
       else run_emit_local<K, VTMAX, 0>(d, nanm, n_mine, cur, phase, out, (done + v0) / K, step, mul, off);
 #pragma unroll
       for (int j = 0; j < K; ++j) carry[j] = ((total.rst >> j) & 1u) ? total.sum[j] : wadd32(carry[j], total.sum[j]);
-      TRACE(5);
       __syncthreads();  // tile_bytes / start16 / sh are reused by the next tile; ostage is complete
       // the staged floats leave while the next tile is loaded and ranked (ostage is not written again before the
       // barriers of the next tile's scans)
       if (dense) copy_out_dense(ostage, out, done, take);
       done += take;
-      TRACE(6);
     }
     if (done < V && threadIdx.x == 0) report_frame_error(L, fidx, DEV_ERR_TRUNCATED);  // v4_codec.cpp:102-104
   }

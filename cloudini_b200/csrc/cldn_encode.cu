@@ -482,16 +482,6 @@ cudaError_t raise_smem_limit_ptr(const void* kernel, size_t bytes) {
 template <typename K>
 static cudaError_t set_smem(K* kernel, size_t bytes) { return raise_smem_limit(kernel, bytes); }
 
-// Tuning variant of the FloatN kernel: 0 = I=8 / 2 CTAs per SM (128 regs), 1 = I=8 / 3 CTAs (80 regs),
-// 2 = I=4 / 4 CTAs (64 regs). Chosen once per process (env CLDN_B200_ENC_VARIANT overrides the default).
-static int floatn_variant() {
-  static const int v = [] {
-    const char* e = getenv("CLDN_B200_ENC_VARIANT");
-    return (e && e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 1;
-  }();
-  return v;
-}
-
 template <int N, int I, int MINB>
 static int launch_floatn(const Plan& plan, const EncLaunch& L, bool vec4, cudaStream_t stream) {
   FloatNParams P;
@@ -580,49 +570,9 @@ __global__ void __launch_bounds__(kGorillaThreads) gorilla_prepass_kernel(const 
   }
 }
 
-// Gorilla pre-pass, one-thread-per-chunk version (CLDN_B200_UNMEASURED=0 only): one thread per (chunk, Gorilla op) walks its 32768 points in order (the window of the previous
-// "new window" record is inherently sequential) and leaves a 12-byte record per point: bytes 0..9 the encoded value,
-// byte 11 its length. The generic kernel then copies the record like any other field. Side layout: [op][point][12].
-__global__ void gorilla_prepass_seq_kernel(const EncLaunch L) {
-  const EncFrame F = L.frames[blockIdx.x];
-  const Plan& plan = *L.plan;
-  const uint32_t items = F.n_chunks * plan.n_gorilla;
-  for (uint32_t it = threadIdx.x; it < items; it += blockDim.x) {
-    const uint32_t chunk = it / plan.n_gorilla, g = it % plan.n_gorilla;
-    uint32_t seen = 0, offset = 0;
-    for (uint32_t k = 0; k < plan.n_ops; ++k) {
-      if (plan.ops[k].kind == OP_GORILLA64) {
-        if (seen == g) offset = plan.ops[k].offset[0];
-        ++seen;
-      }
-    }
-    const uint32_t p0 = chunk * kChunkPoints;
-    const uint32_t n = min(kChunkPoints, F.n_points - p0);
-    uint8_t* side = const_cast<uint8_t*>(F.side) + (static_cast<size_t>(g) * F.n_points + p0) * 12;
-    GorillaState st;
-    st.reset();
-    for (uint32_t i = 0; i < n; ++i) {
-      const uint64_t cur = load_u64(F.in + static_cast<size_t>(p0 + i) * plan.point_step + offset);
-      uint8_t rec[12];
-      const uint32_t len = gorilla_encode(st, cur, rec);
-      for (uint32_t b = 0; b < len; ++b) side[i * 12 + b] = rec[b];
-      side[i * 12 + 11] = static_cast<uint8_t>(len);
-    }
-  }
-}
-
-// The parallel boundary-search decoders, the warp-parallel Gorilla pre-pass and the parallel run-table reader are the
-// defaults (hardware-green since the start of round 2: GPU suite with and without them, gpurun_out/r2_start).
-// CLDN_B200_UNMEASURED=0 selects the older one-thread-per-chunk versions again (bisecting aid).
-bool unmeasured_kernels_enabled() {
-  const char* e = getenv("CLDN_B200_UNMEASURED");
-  return !(e && e[0] == '0');
-}
-
 int launch_gorilla_prepass(const Plan& plan, const EncLaunch& L, cudaStream_t stream) {
   if (plan.n_gorilla == 0 || L.n_frames == 0) return 0;
-  if (unmeasured_kernels_enabled()) gorilla_prepass_kernel<<<L.n_frames, kGorillaThreads, 0, stream>>>(L);
-  else gorilla_prepass_seq_kernel<<<L.n_frames, 64, 0, stream>>>(L);
+  gorilla_prepass_kernel<<<L.n_frames, kGorillaThreads, 0, stream>>>(L);
   count_launch();
   return 1;
 }
@@ -642,7 +592,7 @@ uint32_t choose_tile_points(const Plan& plan) {
     PointsParams pp;
     if (encode_points_applies(plan, &pp)) return encode_points_tile(plan);
   }
-  if (plan.floatn_only) return floatn_variant() == 2 ? kThreads * 4 : kThreads * 8;
+  if (plan.floatn_only) return kThreads * 8;
   const size_t budget = 96 * 1024;
   for (int I = 8; I >= 1; I >>= 1) {
     if (static_cast<size_t>(kThreads) * I * plan.max_point_bytes + sizeof(Plan) + 64 <= budget) return kThreads * I;
@@ -678,18 +628,9 @@ int launch_encode_regular(const Plan& plan, const EncLaunch& L, cudaStream_t str
     const bool packed4 = op.lanes == 4 && plan.point_step == 16 && op.offset[0] == 0 && op.offset[1] == 4 &&
                          op.offset[2] == 8 && op.offset[3] == 12;
     const bool vec4 = packed4 && (L.flags & kEncInputsAligned16);  // LDG.128 needs 16-byte aligned frame bases
-    const int variant = floatn_variant();
-    if (L.tile_points != (variant == 2 ? kThreads * 4 : kThreads * 8)) return -1;
-    if (op.lanes == 4) {
-      if (variant == 0) return launch_floatn<4, 8, 2>(plan, L, vec4, stream);
-      if (variant == 1) return launch_floatn<4, 8, 3>(plan, L, vec4, stream);
-      if (variant == 3) return launch_floatn<4, 8, 4>(plan, L, vec4, stream);
-      return launch_floatn<4, 4, 4>(plan, L, vec4, stream);
-    }
-    if (variant == 0) return launch_floatn<3, 8, 2>(plan, L, false, stream);
-    if (variant == 1) return launch_floatn<3, 8, 3>(plan, L, false, stream);
-    if (variant == 3) return launch_floatn<3, 8, 4>(plan, L, false, stream);
-    return launch_floatn<3, 4, 4>(plan, L, false, stream);
+    if (L.tile_points != kThreads * 8) return -1;
+    if (op.lanes == 4) return launch_floatn<4, 8, 3>(plan, L, vec4, stream);
+    return launch_floatn<3, 8, 3>(plan, L, false, stream);
   }
   const EncLaunch& LL = L;
   const uint32_t I = LL.tile_points / kThreads;

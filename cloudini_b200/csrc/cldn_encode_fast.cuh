@@ -21,14 +21,9 @@
 #pragma once
 
 namespace cldn {
-#ifndef CLDN_FAST_ENC_POLL_IN_PASS2
-#define CLDN_FAST_ENC_POLL_IN_PASS2 0   // 1 = warp 0 polls its look-back window between points of pass 2 (measured slightly slower)
-#endif
-#ifndef CLDN_FAST_ENC_MINB
-#define CLDN_FAST_ENC_MINB 6
-#endif
 
 constexpr int kET = 128;                  // threads per CTA
+constexpr int kFastEncMinBlocks = 6;      // resident CTAs per SM the register allocation aims at
 constexpr int kEW = kET / 32;
 constexpr int kEP = 8;                    // points per thread and tile
 constexpr int kETilePts = kET * kEP;      // 1024
@@ -154,7 +149,7 @@ __device__ __forceinline__ void tile_coords(const EncLaunch& L, uint32_t i, uint
   }
 }
 
-__global__ void __launch_bounds__(kET, CLDN_FAST_ENC_MINB) encode_xyzi_fast_kernel(const EncLaunch L, const FloatNParams P) {
+__global__ void __launch_bounds__(kET, kFastEncMinBlocks) encode_xyzi_fast_kernel(const EncLaunch L, const FloatNParams P) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   __shared__ EncFastShared sh;
   __shared__ EncFrame s_F[2];
@@ -349,11 +344,6 @@ __global__ void __launch_bounds__(kET, CLDN_FAST_ENC_MINB) encode_xyzi_fast_kern
           if (wn != wa) { *reinterpret_cast<uint32_t*>(stage + wa) = lo; lo = hi; }
           wa = wn;
         }
-#if CLDN_FAST_ENC_POLL_IN_PASS2
-        // warp 0 looks at its look-back window between points: the tile's inclusive prefix is published as soon as the
-        // predecessors allow, not only after this warp's share of the packing
-        if (warp == 0 && (j & 1) == 1) lb.poll_once(L.status, F.tile_begin, tile, L.epoch, total);
-#endif
       }
       if (threadIdx.x == kET - 1 && (bit & 31u) != 0u) *reinterpret_cast<uint32_t*>(stage + wa) = lo;  // nobody follows the tile's last thread
     } else {

@@ -26,10 +26,6 @@ struct PointsParams {
   uint32_t point_step;
 };
 
-#ifndef CLDN_POINTS_CPASYNC
-#define CLDN_POINTS_CPASYNC 1   // tile bytes by cp.async (0: ld.global.cs + st.shared)
-#endif
-
 // Field reads from the staged tile. On the device the address is a 32-bit shared-window address and the loads are
 // ld.shared: through a generic `const uint8_t*` every read cost 64-bit pointer arithmetic and a generic load (17
 // instructions per value measured; the kernel is instruction-bound).
@@ -98,13 +94,8 @@ __global__ void __launch_bounds__(kPT) encode_points_fast_kernel(const EncLaunch
     const uint32_t nvec = (bytes - head) >> 4;
     const uint4* gv = reinterpret_cast<const uint4*>(g + head);
     uint4* sv = reinterpret_cast<uint4*>(s + head);
-#if CLDN_POINTS_CPASYNC
     for (uint32_t i = threadIdx.x; i < nvec; i += kPT) async_copy16(sv + i, gv + i);   // cp.async: no register round trip
     async_commit();
-#else
-#pragma unroll 4
-    for (uint32_t i = threadIdx.x; i < nvec; i += kPT) sv[i] = __ldcs(gv + i);
-#endif
     const uint32_t done = head + 16u * nvec;
     if (threadIdx.x < bytes - done) s[done + threadIdx.x] = g[done + threadIdx.x];
     async_wait_all();
@@ -285,10 +276,8 @@ static uint32_t encode_points_values(const Plan& plan) {
   for (uint32_t i = 0; i < plan.n_ops; ++i) nv += plan.ops[i].kind == OP_FLOATN ? plan.ops[i].lanes : 1u;
   return nv;
 }
-#ifndef CLDN_POINTS_EP_WIDE
-#define CLDN_POINTS_EP_WIDE 4   // points per thread for 5 / 6 values per point (8: 40-48 values in registers)
-#endif
-static uint32_t encode_points_tile(const Plan& plan) { return encode_points_values(plan) <= 4 ? kPT * 8 : kPT * CLDN_POINTS_EP_WIDE; }
+constexpr int kPointsWideEP = 4;   // points per thread for 5 / 6 values per point (8: 40-48 values in registers)
+static uint32_t encode_points_tile(const Plan& plan) { return encode_points_values(plan) <= 4 ? kPT * 8 : kPT * kPointsWideEP; }
 
 template <int NV, int EP, int NF>
 static int launch_points_nf(const Plan& plan, const EncLaunch& L, const PointsParams& P, cudaStream_t stream) {
@@ -330,8 +319,8 @@ static int launch_encode_points(const Plan& plan, const EncLaunch& L, const Poin
   switch (encode_points_values(plan)) {
     case 3: return launch_points_nv<3, 8>(plan, L, P, stream);
     case 4: return launch_points_nv<4, 8>(plan, L, P, stream);
-    case 5: return launch_points_nv<5, CLDN_POINTS_EP_WIDE>(plan, L, P, stream);
-    default: return launch_points_nv<6, CLDN_POINTS_EP_WIDE>(plan, L, P, stream);
+    case 5: return launch_points_nv<5, kPointsWideEP>(plan, L, P, stream);
+    default: return launch_points_nv<6, kPointsWideEP>(plan, L, P, stream);
   }
 }
 

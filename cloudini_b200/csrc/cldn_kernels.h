@@ -73,7 +73,6 @@ struct DecLaunch {
   uint32_t* tile_chunk;        // per tile: global chunk index
   uint64_t* tstatus;           // per tile: look-back 1 (value counts)
   uint32_t* tsums;             // per tile: 2 x 8 words, look-back 2 (aggregate record, inclusive record)
-  uint64_t* trace;             // optional (CLDN_B200_TRACE): 8 globaltimer stamps per tile
   uint32_t* chunk_counter;     // 4 words, zeroed per launch: [0] chunk claims, [1] redo claims, [2] walk ticket, [3] redo count
   uint32_t* redo_list;         // chunks the fast chunk-sequential kernel handed to the careful one (n_chunks_total entries)
   uint32_t redo_mode;          // careful kernel: 1 = decode exactly the chunks of redo_list (descriptors are already published)
@@ -85,8 +84,6 @@ struct DecLaunch {
   uint32_t tile_capacity;      // records allocated (== tile_grid)
   uint32_t tile_grid;          // host upper bound on the number of tiles
   uint32_t epoch;
-  uint32_t mix_chase;          // decode_mixed_kernel: 1 = one thread follows next() through the tile instead of pointer doubling
-  uint32_t par_runs;           // V5 Rle / DeltaRle readers: 1 = parallel run-table parse (see unmeasured_kernels_enabled)
   // Side mode (V5 sections decoded AHEAD of the regular stream, large batches): stream_end_kernel finds where every chunk's
   // regular stream ends, the section reader writes its values into compact arrays -- section s of global chunk gc at
   // side + side_off[s] + gc * kChunkPoints * bpv -- and the fast reader merges them into the rows it writes, so that
@@ -105,10 +102,6 @@ template <class Launch>
 __device__ __forceinline__ uint32_t* frame_err_word(const Launch& L, uint32_t f) { return L.frame_err ? L.frame_err + f : L.err; }
 template <class Launch>
 __device__ __forceinline__ void report_frame_error(const Launch& L, uint32_t f, uint32_t code) { atomicCAS(frame_err_word(L, f), 0u, code); }
-
-// The parallel boundary-search decoders, the warp-parallel Gorilla pre-pass and the parallel run-table parse: defaults
-// since round 2 (hardware-green); CLDN_B200_UNMEASURED=0 selects the older one-thread-per-chunk versions (bisecting aid).
-bool unmeasured_kernels_enabled();
 
 int launch_decode(const Plan& host_plan, const DecLaunch& L, cudaStream_t stream);
 int launch_decode_tiles(const Plan& host_plan, const DecLaunch& L, cudaStream_t stream);
@@ -140,7 +133,6 @@ struct SecLaunch {
   uint64_t* hash_scratch;        // palette hash tables
   uint32_t* err;
   uint32_t header_bytes;
-  uint32_t staged;               // set by launch_encode_sections: fields of <= 4 bytes are taken by encode_sections_staged_kernel
 };
 int launch_encode_sections(const Plan& host_plan, const SecLaunch& L, cudaStream_t stream);
 size_t palette_overflow_scratch_bytes();

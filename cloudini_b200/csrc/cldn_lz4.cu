@@ -31,10 +31,7 @@ constexpr int kLzThreads = 128;          // 4 warps = 4 chunks per CTA
 constexpr int kLzWarps = kLzThreads / 32;
 constexpr uint32_t kLzHashBits = 11;    // 2048 entries of (16-bit tag << 16 | 16-bit position) per warp = 8 KB
 constexpr int kLzR = 4;                  // positions per lane and step of the compressor
-#ifndef CLDN_LZ4_MIN_MATCH
-#define CLDN_LZ4_MIN_MATCH 6
-#endif
-constexpr int kLzMinMatch = CLDN_LZ4_MIN_MATCH;   // 4 (the format's minimum) .. 8: shortest match the compressor takes.
+constexpr int kLzMinMatch = 6;           // 4 (the format's minimum) .. 8: shortest match the compressor takes.
 // Sizes on config 4 (1000 x 130 048-point XYZI frames, 6.802 stage-1 bytes per point; liblz4: 6.61): minimum match
 //   5: 6.747 B per point    6: 6.797    8: 6.825 (the block framing outweighs the matches). Shorter minimum matches were
 // slower to encode and decode; 6 never expands and was close to 8 in time.

@@ -435,7 +435,7 @@ __global__ void __launch_bounds__(kSecThreads, 1) encode_sections_kernel(const S
   const Plan& plan = *L.plan;
   const uint32_t ns = plan.n_sections;
   const uint32_t gc = blockIdx.x / ns, s = blockIdx.x % ns;
-  if (L.staged && plan.sections[s].bpv <= 4) return;  // encode_sections_staged_kernel
+  if (plan.sections[s].bpv <= 4) return;  // encode_sections_staged_kernel
   const uint32_t f = L.chunk_frame[gc];
   const EncFrame F = L.frames[f];
   const uint32_t chunk = gc - L.chunk_first[f];
@@ -820,26 +820,23 @@ int launch_encode_sections(const Plan& plan, const SecLaunch& L, cudaStream_t st
   if (raise_smem_limit(encode_sections_kernel, smem) != cudaSuccess) return -1;
   if (raise_smem_limit(palette_overflow_kernel, smem) != cudaSuccess) return -1;
   // fields of <= 4 bytes: the staged writers (values loaded once into shared memory); 64-bit fields: the writers that
-  // read the cloud in place. CLDN_B200_SECTIONS_STAGED=0 sends everything to the latter (bisecting aid).
-  static const bool staged_on = [] { const char* e = getenv("CLDN_B200_SECTIONS_STAGED"); return !(e && e[0] == '0'); }();
+  // read the cloud in place
   bool any_small = false, any_wide = false;
   for (uint32_t s = 0; s < plan.n_sections; ++s) (plan.sections[s].bpv <= 4 ? any_small : any_wide) = true;
-  SecLaunch L2 = L;
-  L2.staged = staged_on ? 1u : 0u;
   int launched = 3;
-  probe_modes_kernel<<<L.n_frames * plan.n_sections, kSecThreads, smem, stream>>>(L2);
-  if (staged_on && any_small) {
+  probe_modes_kernel<<<L.n_frames * plan.n_sections, kSecThreads, smem, stream>>>(L);
+  if (any_small) {
     const size_t smem2 = sizeof(StagedShared) + 16;
     if (raise_smem_limit(encode_sections_staged_kernel, smem2) != cudaSuccess) return -1;
-    encode_sections_staged_kernel<<<L.n_chunks_total * plan.n_sections, kSecThreads, smem2, stream>>>(L2);
+    encode_sections_staged_kernel<<<L.n_chunks_total * plan.n_sections, kSecThreads, smem2, stream>>>(L);
     ++launched;
   }
-  if (!staged_on || any_wide) {
-    encode_sections_kernel<<<L.n_chunks_total * plan.n_sections, kSecThreads, smem, stream>>>(L2);
+  if (any_wide) {
+    encode_sections_kernel<<<L.n_chunks_total * plan.n_sections, kSecThreads, smem, stream>>>(L);
     ++launched;
   }
-  palette_overflow_kernel<<<kOverflowTables, kSecThreads, smem, stream>>>(L2);
-  scan_sections_kernel<<<(L.n_frames * 32 + 127) / 128, 128, 0, stream>>>(L2);
+  palette_overflow_kernel<<<kOverflowTables, kSecThreads, smem, stream>>>(L);
+  scan_sections_kernel<<<(L.n_frames * 32 + 127) / 128, 128, 0, stream>>>(L);
   count_launch(launched);
   return launched;
 }

@@ -194,11 +194,6 @@ def build(force=False, opt="-O1", asan=False):
     """asan=True builds libcloudini_b200_cusim_asan.so (AddressSanitizer: out-of-bounds accesses of the kernels on
     "device" = heap memory are reported). Load it with LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0."""
     lib = LIB.replace(".so", "_asan.so") if asan else LIB
-    # CUSIM_DEFINES="A=1 B=2": emulate a build variant of the kernels (development: a variant is checked here before it costs GPU time)
-    defines = os.environ.get("CUSIM_DEFINES", "").split()
-    if defines:
-        lib = lib.replace(".so", "_" + "_".join(defines).replace("=", "") + ".so")
-        force = True
     if not force and not asan and not needs_build():
         return LIB
     os.makedirs(GEN, exist_ok=True)
@@ -207,7 +202,7 @@ def build(force=False, opt="-O1", asan=False):
             text = fh.read()
         with open(os.path.join(GEN, f), "w") as fh:
             fh.write(transform(text, f))
-    flags = ["-std=c++17", opt, "-g", "-fPIC", "-ffp-contract=off", "-fno-strict-aliasing", "-pthread", "-I", HERE, "-w"] + ["-D" + d for d in defines]
+    flags = ["-std=c++17", opt, "-g", "-fPIC", "-ffp-contract=off", "-fno-strict-aliasing", "-pthread", "-I", HERE, "-w"]
     if asan:
         # + alignment: x86 tolerates a misaligned uint4 / uint64 access, the GPU raises "misaligned address"
         # + shift-exponent / float-cast-overflow / integer-divide-by-zero: where C++ leaves the result open the two
@@ -218,7 +213,7 @@ def build(force=False, opt="-O1", asan=False):
     procs = []
     for src in SOURCES + ["cusim.cpp"]:
         path = os.path.join(HERE, src) if src == "cusim.cpp" else os.path.join(GEN, src)
-        obj = os.path.join(OUT_DIR, os.path.splitext(src)[0] + ("_asan.o" if asan else "_var.o" if defines else ".o"))
+        obj = os.path.join(OUT_DIR, os.path.splitext(src)[0] + ("_asan.o" if asan else ".o"))
         cmd = ["g++", *flags, "-x", "c++", "-c", path, "-o", obj]
         procs.append((src, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     objs = []

@@ -26,7 +26,7 @@ for name in only:
     blob = ref.encode(info, cloud)
     dinfo, hdr = cb.DecodeHeader(blob)
     n = cloud.size
-    modes = [("CLDN_B200_DECODE_MODE", m) for m in ("seq", "tile")] if name.startswith(("c2", "c1")) else [("CLDN_B200_MIXED_DECODE", m) for m in ("par", "chase", "seq")]
+    modes = [("CLDN_B200_DECODE_MODE", m) for m in ("seq", "tile")] if name.startswith(("c2", "c1")) else [("CLDN_B200_MIXED_DECODE", m) for m in ("par", "seq")]
     mm = 0
     for t in range(trials):
         b = bytearray(blob)

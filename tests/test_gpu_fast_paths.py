@@ -322,29 +322,26 @@ def _int_sections_layout(n, seed, with_u64=False, only_u64=False):
     return info, raw.reshape(-1)
 
 
-@pytest.mark.parametrize("holes", ["0", "1"])
+@pytest.mark.parametrize("shift", [0, 2])
 @pytest.mark.parametrize("n", [1, 9, 1024, 4097, 32768, 32769, 70_001])
-def test_sections_ahead_same_bytes_as_sections_behind(oracle, monkeypatch, n, holes):
-    """holes = 1: padded layouts leave the fast reader as whole rows over a copy of the old rows (opt-in: measured slower)."""
+def test_sections_ahead_same_bytes_as_sections_behind(oracle, monkeypatch, n, shift):
     monkeypatch.setenv("CLDN_B200_DECODE_MODE", "seq")
-    monkeypatch.setenv("CLDN_B200_DECODE_ROWS_HOLES", holes)
     cases = [synth.cloud_c3(n, seed=n, version=5), _xyzirt(n, 3), _int_sections_layout(n, n), _int_sections_layout(n, n + 1, only_u64=True)]
     for info, cloud in cases:
         step = info.point_step
         clouds = [cloud, np.ascontiguousarray(cloud.reshape(n, step)[::-1]).reshape(-1)]
         blobs, hdr = _encode_all(info, clouds, oracle)
-        for shift in (0, 2):
-            seen = {}
-            for flag in ("1", "0"):
-                monkeypatch.setenv("CLDN_B200_DECODE_SIDE", flag)
-                outs, (fast, redo), ahead = _decode_batch_side(info, blobs, hdr, n * step, 0x5C, shift)
-                assert ahead == (flag == "1"), (n, flag)
-                assert (fast, redo) == (2 * ((n + 32767) // 32768), 0), (n, flag, fast, redo)
-                seen[flag] = outs
-            for b, o1, o0 in zip(blobs, seen["1"], seen["0"]):
-                want = _want(oracle, b, n * step, 0x5C)
-                assert np.array_equal(o1, want), (n, shift)
-                assert np.array_equal(o0, want), (n, shift)
+        seen = {}
+        for flag in ("1", "0"):
+            monkeypatch.setenv("CLDN_B200_DECODE_SIDE", flag)
+            outs, (fast, redo), ahead = _decode_batch_side(info, blobs, hdr, n * step, 0x5C, shift)
+            assert ahead == (flag == "1"), (n, flag)
+            assert (fast, redo) == (2 * ((n + 32767) // 32768), 0), (n, flag, fast, redo)
+            seen[flag] = outs
+        for b, o1, o0 in zip(blobs, seen["1"], seen["0"]):
+            want = _want(oracle, b, n * step, 0x5C)
+            assert np.array_equal(o1, want), (n, shift)
+            assert np.array_equal(o0, want), (n, shift)
 
 
 def test_sections_ahead_with_chunks_for_the_careful_kernels(oracle, monkeypatch):

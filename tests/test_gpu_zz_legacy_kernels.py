@@ -1,7 +1,7 @@
-"""The one-thread-per-chunk kernels that were the defaults in round 1 (sequential Gorilla pre-pass, decode_sequential_kernel
-for raw / XOR / Gorilla streams, the thread-0 run-table parser) stay selectable with CLDN_B200_UNMEASURED=0 as a bisecting
-aid; the parallel replacements are the defaults since they went hardware-green at the start of round 2. This file keeps
-the old path honest: every test re-runs a parity test of test_gpu_parity.py / test_gpu_ros.py with the switch off.
+"""decode_sequential_kernel -- the one-thread-per-chunk parser of raw / XOR / Gorilla streams -- on the plans that the
+parallel boundary searches (decode_mixed_kernel, decode_gorilla_kernel) take by default. The sequential parser stays
+because overlapping fields and two or more Gorilla fields need it; CLDN_B200_MIXED_DECODE=seq sends every such plan to
+it. Every test here re-runs a parity test of test_gpu_parity.py / test_gpu_ros.py with that switch set.
 It sorts last on purpose (a surprise here cannot hide the defaults' results behind `pytest -x`)."""
 import os
 import sys
@@ -17,8 +17,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True)
 def _legacy_kernels(monkeypatch):
-    monkeypatch.setenv("CLDN_B200_UNMEASURED", "0")
-    monkeypatch.delenv("CLDN_B200_MIXED_DECODE", raising=False)
+    monkeypatch.setenv("CLDN_B200_MIXED_DECODE", "seq")
 
 
 def test_golden_vectors(golden, oracle):            # v2 goldens: XOR / Gorilla coders of the reference, wire versions 3 / 4 / 5
@@ -27,7 +26,7 @@ def test_golden_vectors(golden, oracle):            # v2 goldens: XOR / Gorilla 
 
 @pytest.mark.parametrize("version", [5, 4, 3])
 @pytest.mark.parametrize("lossless", [True, False])
-def test_lossless_float_fields(oracle, version, lossless):   # sequential Gorilla pre-pass + decode_sequential_kernel
+def test_lossless_float_fields(oracle, version, lossless):
     P.test_lossless_float_fields(oracle, version, lossless)
 
 
@@ -39,19 +38,6 @@ def test_raw_fields_in_the_stream(oracle, monkeypatch, mode, version):
 
 def test_gorilla_field_positions(oracle, monkeypatch):
     P.test_gorilla_field_positions(oracle, monkeypatch, "seq")
-
-
-def test_v5_long_run_tables(oracle):                 # thread-0 Rle / DeltaRle run-table parse
-    P.test_v5_long_run_tables(oracle)
-
-
-@pytest.mark.parametrize("n", [63, 4097, 32775, 100_003])
-def test_c3_padded_mixed_sizes(oracle, n):
-    P.test_c3_padded_mixed_sizes(oracle, n)
-
-
-def test_v5_all_modes_and_types(oracle):
-    P.test_v5_all_modes_and_types(oracle)
 
 
 def test_v5_section_decode_errors():

@@ -25,21 +25,15 @@ def run(name, info, clouds, reps=10):
     sizes = enc.encode_batch_device(eb, True, want_sizes=True)
     hdr = len(enc.getHeader())
     res = {"case": name, "frames": F, "points": n, "point_step": step, "stage1_B_per_pt": (float(np.mean(sizes)) - hdr) / n}
-    for label, flag in (("encode_ms", None), ("encode_unmeasured_ms", "1")):  # the second: warp-parallel Gorilla pre-pass
-        if flag:
-            os.environ["CLDN_B200_UNMEASURED"] = flag
-        else:
-            os.environ.pop("CLDN_B200_UNMEASURED", None)
+    enc.encode_batch_device(eb, True)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
         enc.encode_batch_device(eb, True)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        for _ in range(reps):
-            enc.encode_batch_device(eb, True)
-        enc.sync()
-        res[label] = (time.perf_counter() - t0) / reps * 1e3
-    os.environ.pop("CLDN_B200_UNMEASURED", None)
+    enc.sync()
+    res["encode_ms"] = (time.perf_counter() - t0) / reps * 1e3
     outs = {}
-    for mode in ("par", "chase", "seq"):
+    for mode in ("par", "seq"):
         os.environ["CLDN_B200_MIXED_DECODE"] = mode
         dec = cb.PointcloudDecoder()
         db = dec.make_device_batch([t.data_ptr() + hdr for t in d_blob], [x - hdr for x in sizes], [t.data_ptr() for t in d_out], [n * step] * F)
@@ -51,7 +45,7 @@ def run(name, info, clouds, reps=10):
             dec.decode_batch_device(info, db, sync=False)
         dec.sync()
         res[f"decode_{mode}_ms"] = (time.perf_counter() - t0) / reps * 1e3
-    res["modes_agree"] = bool(np.array_equal(outs["par"], outs["seq"]) and np.array_equal(outs["chase"], outs["seq"]))
+    res["modes_agree"] = bool(np.array_equal(outs["par"], outs["seq"]))
     print(json.dumps(res), flush=True)
 
 
