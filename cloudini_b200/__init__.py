@@ -29,6 +29,7 @@ CLDN_MAX_FIELDS = 32
 CLDN_MAX_NAME = 64
 kDecodeButSkipStore = 0xFFFFFFFF  # basic_types.hpp:71
 MEM_HOST, MEM_DEVICE = 0, 1
+MEM_DEVICE_POINTS = 2  # points (clouds, decoded outputs) in device memory, blobs and payloads in host memory
 
 
 class FieldType(enum.IntEnum):  # basic_types.hpp:29-48
@@ -365,15 +366,9 @@ class PointcloudEncoder:
         import numpy as np
         n = len(clouds)
         m = max(n, 1)
-        step = self._info.point_step
         widths, heights = self._dims(n, dims)
         ins = [_host_ptr(c) for c in clouds]
-        caps = []
-        for k, (_, nbytes, _) in enumerate(ins):
-            pts = nbytes // step if step else 0
-            w, h = dims[k] if dims is not None else (pts, 1)
-            # a cloud that is not a whole number of points gets a 1-byte buffer: the library reports the frame
-            caps.append(MaxCompressedSize(replace(self._info, width=int(w), height=int(h)), pts, True) if step and nbytes % step == 0 else 1)
+        caps = [self._blob_cap(nbytes, dims[k] if dims is not None else None) for k, (_, nbytes, _) in enumerate(ins)]
         outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps]
         written = (C.c_size_t * m)()
         _check(lib().cldn_b200_encode_blobs(self._h, n, (C.c_void_p * m)(*[p[0] for p in ins]), (C.c_size_t * m)(*[p[1] for p in ins]),
@@ -393,6 +388,46 @@ class PointcloudEncoder:
         _check(lib().cldn_b200_encode_blobs(self._h, n, (C.c_void_p * m)(*in_ptrs), (C.c_size_t * m)(*in_bytes), widths, heights,
                                             (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps), written, MEM_DEVICE))
         return [int(written[f]) for f in range(n)] if want_sizes else None
+
+    def _blob_cap(self, nbytes: int, dims=None) -> int:
+        """Capacity of the blob of a cloud of `nbytes` for encode_blobs / encode_blobs_from_device: MaxCompressedSize with
+        the header of its dims ((width, height), None for (points, 1)), or 1 byte for a cloud that is not a whole number
+        of points, which the library then reports as that frame's error."""
+        step = self._info.point_step
+        if not step or nbytes % step:
+            return 1
+        w, h = dims if dims is not None else (nbytes // step, 1)
+        return MaxCompressedSize(replace(self._info, width=int(w), height=int(h)), nbytes // step, True)
+
+    def encode_device(self, ptr: int, nbytes: int, write_header: bool = True) -> bytes:
+        """encode() of a device-resident cloud (a device address of `nbytes`): the blob comes back in host memory, as
+        encode() writes it. The cloud is read on this encoder's stream."""
+        import numpy as np
+        if self._info.point_step == 0:
+            raise RuntimeError("point_step cannot be 0")
+        if nbytes % self._info.point_step:
+            raise RuntimeError("Input cloud_data size is not a multiple of point_step")
+        cap = MaxCompressedSize(self._info, nbytes // self._info.point_step, True)
+        out = np.empty(max(cap, 1), dtype=np.uint8)
+        written = C.c_size_t(0)
+        _check(lib().cldn_b200_encode(self._h, ptr, nbytes, out.ctypes.data, cap, 1 if write_header else 0, C.byref(written),
+                                      MEM_DEVICE_POINTS))
+        return out[:written.value].tobytes()
+
+    def encode_blobs_from_device(self, in_ptrs: Sequence[int], in_bytes: Sequence[int], dims: Optional[Sequence] = None) -> List[bytes]:
+        """encode_blobs() of device-resident clouds (device addresses): complete blobs in host memory, byte-identical to
+        what encode_blobs() gives the same clouds in host memory."""
+        import numpy as np
+        n = len(in_ptrs)
+        m = max(n, 1)
+        widths, heights = self._dims(n, dims)
+        caps = [self._blob_cap(int(b), dims[f] if dims is not None else None) for f, b in enumerate(in_bytes)]
+        outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps]
+        written = (C.c_size_t * m)()
+        _check(lib().cldn_b200_encode_blobs(self._h, n, (C.c_void_p * m)(*in_ptrs), (C.c_size_t * m)(*in_bytes), widths, heights,
+                                            (C.c_void_p * m)(*[o.ctypes.data for o in outs]), (C.c_size_t * m)(*caps), written,
+                                            MEM_DEVICE_POINTS))
+        return [outs[f][:written[f]].tobytes() for f in range(n)]
 
     def sizes_device_ptr(self) -> int:
         return int(lib().cldn_b200_encoder_sizes_device(self._h) or 0)
@@ -492,6 +527,25 @@ class PointcloudDecoder:
         m = max(n, 1)
         return self._blobs(n, (C.c_void_p * m)(*ptrs), (C.c_size_t * m)(*sizes), (C.c_void_p * m)(*out_ptrs),
                            (C.c_size_t * m)(*out_caps), MEM_DEVICE)
+
+    def decode_to_device(self, info: EncodingInfo, payload, out_ptr: int, out_cap: int):
+        """decode() of a host payload (no header) into a device buffer of `out_cap` bytes at device address `out_ptr`,
+        in place: only declared field bytes are written. Ordered on this decoder's stream; synchronous."""
+        addr, nbytes, keep = _host_ptr(payload)
+        c = _to_c(info)
+        _check(lib().cldn_b200_decode(self._h, C.byref(c), addr, nbytes, out_ptr, out_cap, MEM_DEVICE_POINTS))
+        del keep
+
+    def decode_blobs_to_device(self, blobs: Sequence, out_ptrs: Sequence[int], out_caps: Sequence[int]):
+        """decode_blobs() of host blobs into device buffers (device addresses). Returns (statuses, EncodingInfos) as
+        decode_blobs_device() does; statuses and frame_error(f) are those decode_blobs() gives the same blobs."""
+        n = len(blobs)
+        m = max(n, 1)
+        ins = [_host_ptr(b) for b in blobs]
+        r = self._blobs(n, (C.c_void_p * m)(*[p[0] for p in ins]), (C.c_size_t * m)(*[p[1] for p in ins]),
+                        (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps), MEM_DEVICE_POINTS)
+        del ins
+        return r
 
     def frame_error(self, f: int) -> str:
         """Message of frame f of the last decode_blobs / decode_blobs_device ("" when it decoded)."""

@@ -754,7 +754,9 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     if (rc) return rc;
     return read_written(e, n_frames, written_host);
   }
-  if (mem != CLDN_MEM_HOST) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  // CLDN_MEM_DEVICE_POINTS: the host route with the clouds read in place (ordered on the handle's stream, no upload)
+  const bool device_points = mem == CLDN_MEM_DEVICE_POINTS;
   const size_t hdr = write_header ? e->header.size() : 0;
   if (e->stage2 != CLDN_COMP_NONE) {
     if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
@@ -766,10 +768,13 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
       if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
       bool ok;
       size_t cap1 = max_compressed_size(e->info, cloud_bytes[f] / e->info.point_step, false, &ok);
-      if (int rc = e->d_in.reserve(cloud_bytes[f] + 256)) return rc;
       if (int rc = e->d_out.reserve(cap1 + 256)) return rc;
-      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(e->d_in.p, clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
-      const void* din = e->d_in.p;
+      const void* din = clouds[f];
+      if (!device_points) {
+        if (int rc = e->d_in.reserve(cloud_bytes[f] + 256)) return rc;
+        if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(e->d_in.p, clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
+        din = e->d_in.p;
+      }
       void* dout = e->d_out.p;
       if (int rc = encode_batch_device(e, 1, &din, &cloud_bytes[f], &dout, &cap1, 0)) return rc;
       if (int rc = e->h_sizes.reserve(1)) return rc;
@@ -801,16 +806,22 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     }
     caps[f] = std::min(out_capacities[f], worst);
   }
-  std::vector<void*> din, dout;
-  if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, din)) return rc;
+  std::vector<void*> staged, dout;
+  std::vector<const void*> din(clouds, clouds + n_frames);
+  if (!device_points) {
+    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, staged)) return rc;
+    din.assign(staged.begin(), staged.end());
+  }
   if (int rc = stage_layout(e->d_out, n_frames, caps.data(), dout)) return rc;
   if (int rc = e->pipe.ensure(2 * n_frames)) return rc;
   if (int rc = e->h_sizes.reserve(n_frames)) return rc;
   // frame f: upload on the h2d stream -> encode on the handle's stream -> 8-byte size read-back
   for (size_t f = 0; f < n_frames; ++f) {
-    if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(din[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
-    CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f], e->pipe.h2d));
-    CUDA_TRY(cudaStreamWaitEvent(e->stream, e->pipe.ev[2 * f], 0));
+    if (!device_points) {
+      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(staged[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
+      CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f], e->pipe.h2d));
+      CUDA_TRY(cudaStreamWaitEvent(e->stream, e->pipe.ev[2 * f], 0));
+    }
     if (int rc = encode_batch_device(e, 1, &din[f], &cloud_bytes[f], &dout[f], &caps[f], write_header)) return rc;
     CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p + f, e->d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
     CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f + 1], e->stream));
@@ -860,12 +871,12 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   }
   if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (n_frames == 0) return CLDN_OK;
-  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && e->stage2 != CLDN_COMP_LZ4) {
     set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
     return CLDN_ERR_UNSUPPORTED;
   }
-  if (mem == CLDN_MEM_HOST && e->stage2 != CLDN_COMP_NONE && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
+  if (mem != CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
   cldn_info_t full = e->info;
   full.compression_opt = static_cast<uint8_t>(e->stage2);
   std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
@@ -897,7 +908,7 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     payload_cap[f] = out_capacities[f] - h.size();
   }
   CUDA_TRY(cudaSetDevice(e->device));
-  if (mem == CLDN_MEM_HOST) {
+  if (mem != CLDN_MEM_DEVICE) {  // the blobs are host memory (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS)
     std::vector<size_t> w(n_frames, 0);
     if (int rc = encode_batch_impl(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data(), mem)) return rc;
     for (size_t f = 0; f < n_frames; ++f) {
@@ -1381,9 +1392,10 @@ static int stage_padding(const cldn_decoder* d, void* staged, const void* out, s
 }
 
 // Host pointers, compression ZSTD: the payloads go up compressed, the device decompresses and decodes them, the points
-// come back (with the caller's padding bytes, like the uncompressed host path).
+// come back (with the caller's padding bytes, like the uncompressed host path). `device_out` (CLDN_MEM_DEVICE_POINTS):
+// the points are decoded in place into the caller's device buffers and the error word is left to the caller.
 static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
-                                  const size_t* payload_bytes, void* const* outs, const uint64_t* frame_points) {
+                                  const size_t* payload_bytes, void* const* outs, const uint64_t* frame_points, bool device_out) {
   std::vector<void*> din;
   if (int rc = stage_layout(d->d_in, n_frames, payload_bytes, din)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
@@ -1398,6 +1410,7 @@ static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size
   const size_t wh = static_cast<size_t>(info.width) * info.height;
   std::vector<size_t> caps(n_frames);
   for (size_t f = 0; f < n_frames; ++f) caps[f] = static_cast<size_t>(frame_points ? frame_points[f] : wh) * info.point_step;
+  if (device_out) return decode_batch_device(d, plain, n_frames, p1.data(), b1.data(), outs, caps.data(), frame_points);
   std::vector<void*> dout;
   if (int rc = stage_layout(d->d_out, n_frames, caps.data(), dout)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
@@ -1410,10 +1423,12 @@ static int decode_batch_host_zstd(cldn_decoder* d, const cldn_info_t& info, size
   return check_device_error(d->stream, d->d_err.p, d->h_err.p);
 }
 
-// Host pointers, no stage 2. `frame_points` as decode_batch_device takes it.
+// Host pointers, no stage 2. `frame_points` as decode_batch_device takes it. `device_out` (CLDN_MEM_DEVICE_POINTS): the
+// points are decoded in place into the caller's device buffers, and the call returns once the payloads have been read,
+// leaving the error word to the caller.
 static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
                                    const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
-                                   const uint64_t* frame_points) {
+                                   const uint64_t* frame_points, bool device_out) {
   if (int rc = decoder_update_plan(d, info)) return rc;
   const size_t wh = static_cast<size_t>(info.width) * info.height;
   std::vector<size_t> out_need(n_frames);
@@ -1423,12 +1438,19 @@ static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, siz
   }
   std::vector<void*> din, dout;
   if (int rc = stage_layout(d->d_in, n_frames, payload_bytes, din)) return rc;
-  if (int rc = stage_layout(d->d_out, n_frames, out_need.data(), dout)) return rc;
-  if (int rc = d->pipe.ensure(2 * n_frames)) return rc;
+  if (device_out) dout.assign(outs, outs + n_frames);
+  else if (int rc = stage_layout(d->d_out, n_frames, out_need.data(), dout)) return rc;
+  if (int rc = d->pipe.ensure(2 * n_frames + 1)) return rc;
+  // an earlier CLDN_MEM_DEVICE_POINTS call may have returned with its decode still reading the staged payloads on the
+  // handle's stream: whatever this call's memory kind, its uploads into d_in wait for that decode
+  CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * n_frames], d->stream));
+  CUDA_TRY(cudaStreamWaitEvent(d->pipe.h2d, d->pipe.ev[2 * n_frames], 0));
   // frame f: upload on the h2d stream -> decode on the handle's stream -> download on the d2h stream
   for (size_t f = 0; f < n_frames; ++f) {
     if (payload_bytes[f]) CUDA_TRY(cudaMemcpyAsync(din[f], payloads[f], payload_bytes[f], cudaMemcpyHostToDevice, d->pipe.h2d));
-    if (int rc = stage_padding(d, dout[f], outs[f], out_need[f], d->pipe.h2d)) return rc;
+    if (!device_out) {
+      if (int rc = stage_padding(d, dout[f], outs[f], out_need[f], d->pipe.h2d)) return rc;
+    }
     CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f], d->pipe.h2d));
     CUDA_TRY(cudaStreamWaitEvent(d->stream, d->pipe.ev[2 * f], 0));
     const uint64_t* pts = frame_points ? frame_points + f : nullptr;
@@ -1437,9 +1459,14 @@ static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, siz
     const int rc = decode_batch_device(d, info, 1, &din[f], &payload_bytes[f], &dout[f], &out_need[f], pts);
     d->frame_err = group_err;
     if (rc) return rc;
+    if (device_out) continue;
     CUDA_TRY(cudaEventRecord(d->pipe.ev[2 * f + 1], d->stream));
     CUDA_TRY(cudaStreamWaitEvent(d->pipe.d2h, d->pipe.ev[2 * f + 1], 0));
     if (out_need[f]) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], out_need[f], cudaMemcpyDeviceToHost, d->pipe.d2h));
+  }
+  if (device_out) {
+    CUDA_TRY(cudaStreamSynchronize(d->pipe.h2d));  // the payloads have been read
+    return CLDN_OK;
   }
   CUDA_TRY(cudaStreamSynchronize(d->pipe.d2h));
   // a failed decode must not hand back garbage silently: the error word is checked after everything has drained
@@ -1447,8 +1474,8 @@ static int decode_batch_host_plain(cldn_decoder* d, const cldn_info_t& info, siz
 }
 
 // Whether decode_frames decodes frames of `info` in `mem` whole, with an error word per frame (DecLaunch /
-// Lz4Launch::frame_err). The others go frame by frame: LZ4 with host pointers and CLDN_B200_ZSTD_HOST through the host
-// libraries (decode_batch_impl), and compressions that no route decodes.
+// Lz4Launch::frame_err). The others go frame by frame: LZ4 with host payloads and CLDN_B200_ZSTD_HOST through the host
+// libraries (decode_batch_impl), and compressions that no route decodes. CLDN_MEM_DEVICE_POINTS takes the host routes.
 static bool route_has_frame_errors(int mem, const cldn_info_t& info) {
   switch (info.compression_opt) {
     case CLDN_COMP_NONE: return true;
@@ -1460,13 +1487,15 @@ static bool route_has_frame_errors(int mem, const cldn_info_t& info) {
 
 // Frames that share `info`, each with frame_points[f] points (nullptr: info.width * info.height), through the one route
 // of their memory kind and compression: device NONE, LZ4 or ZSTD (stage 2 then one fused stage-1 launch), host plain, or
-// host ZSTD decompressed on the device. Device routes leave the error word to the caller; host routes check it.
+// host ZSTD decompressed on the device. Host payloads (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS) take the host routes.
+// Routes that write device points leave the error word to the caller; routes that write host points check it.
 static int decode_frames(cldn_decoder* d, int mem, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
                          const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
                          const uint64_t* frame_points) {
-  if (mem == CLDN_MEM_HOST) {
-    if (info.compression_opt == CLDN_COMP_ZSTD) return decode_batch_host_zstd(d, info, n_frames, payloads, payload_bytes, outs, frame_points);
-    return decode_batch_host_plain(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, frame_points);
+  if (mem != CLDN_MEM_DEVICE) {
+    const bool device_out = mem == CLDN_MEM_DEVICE_POINTS;
+    if (info.compression_opt == CLDN_COMP_ZSTD) return decode_batch_host_zstd(d, info, n_frames, payloads, payload_bytes, outs, frame_points, device_out);
+    return decode_batch_host_plain(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, frame_points, device_out);
   }
   if (info.compression_opt != CLDN_COMP_LZ4 && info.compression_opt != CLDN_COMP_ZSTD) {
     return decode_batch_device(d, info, n_frames, payloads, payload_bytes, outs, out_capacities, frame_points);
@@ -1492,7 +1521,7 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
     if (sync) return check_device_error(d->stream, d->d_err.p, d->h_err.p);
     return CLDN_OK;
   }
-  if (mem != CLDN_MEM_HOST) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
   // the reference rejects a payload that still carries the header (cloudini.cpp:640-643)
   for (size_t f = 0; f < n_frames; ++f) {
     if (payload_bytes[f] >= 10 && memcmp(payloads[f], "CLOUDINI_V", 10) == 0) {
@@ -1522,12 +1551,14 @@ static int decode_batch_impl(cldn_decoder_t* d, const cldn_info_t* info, size_t 
         if (int rc = stage2_decompress_payload(info->compression_opt, static_cast<const uint8_t*>(payloads[f]), payload_bytes[f], d->s2_tmp, max_body)) return rc;
         const void* p1 = d->s2_tmp.data();
         const size_t b1 = d->s2_tmp.size();
-        if (int rc = decode_batch_impl(d, &plain, 1, &p1, &b1, &outs[f], &out_capacities[f], CLDN_MEM_HOST, 1)) return rc;
+        if (int rc = decode_batch_impl(d, &plain, 1, &p1, &b1, &outs[f], &out_capacities[f], mem, 1)) return rc;
       }
       return CLDN_OK;
     }
   }
-  return decode_frames(d, mem, *info, n_frames, payloads, payload_bytes, outs, out_capacities, nullptr);
+  if (int rc = decode_frames(d, mem, *info, n_frames, payloads, payload_bytes, outs, out_capacities, nullptr)) return rc;
+  if (mem == CLDN_MEM_DEVICE_POINTS && sync) return check_device_error(d->stream, d->d_err.p, d->h_err.p);
+  return CLDN_OK;
 }
 
 // ---- complete blobs, any mix of layouts and sizes (cldn_b200_decode_blobs) -----------------------------------------
@@ -1570,7 +1601,7 @@ static int read_blob_headers(cldn_decoder* d, size_t n, const void* const* blobs
     d->frame_errors[f] = status[f] == CLDN_OK ? "" : cldn_b200_last_error();
     if (status[f] != CLDN_OK) d->frame_infos[f] = cldn_info_t{};
   };
-  if (mem == CLDN_MEM_HOST) {
+  if (mem != CLDN_MEM_DEVICE) {  // host blobs
     for (size_t f = 0; f < n; ++f) parse(f, static_cast<const uint8_t*>(blobs[f]), blob_bytes[f]);
     return CLDN_OK;
   }
@@ -1634,8 +1665,8 @@ static int decode_blob_group(cldn_decoder* d, int mem, const cldn_info_t& info, 
   CUDA_TRY(cudaMemsetAsync(d->d_frame_err.p, 0, n * sizeof(uint32_t), d->stream));
   d->frame_err = d->d_frame_err.p;
   int rc = decode_frames(d, mem, info, n, payloads, payload_bytes, outs, caps, points);
-  // the launch word: errors no frame claimed (the host routes have checked it)
-  if (rc == CLDN_OK && mem == CLDN_MEM_DEVICE) rc = check_device_error(d->stream, d->d_err.p, d->h_err.p);
+  // the launch word: errors no frame claimed (the routes that write host points have checked it)
+  if (rc == CLDN_OK && mem != CLDN_MEM_HOST) rc = check_device_error(d->stream, d->d_err.p, d->h_err.p);
   d->frame_err = nullptr;
   if (rc) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->h_frame_err.p, d->d_frame_err.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, d->stream));
@@ -1672,7 +1703,7 @@ static int decode_blobs_impl(cldn_decoder* d, size_t n, const void* const* blobs
   };
   if (n == 0) return CLDN_OK;
   if (!blobs || !blob_bytes || !outs || !caps) { set_error("null argument"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
-  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE) { set_error("bad mem kind"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
   if (cudaSetDevice(d->device) != cudaSuccess) { set_error("cudaSetDevice failed"); return fail_all(CLDN_ERR_CUDA); }
   std::vector<size_t> hdr;
   if (int rc = read_blob_headers(d, n, blobs, blob_bytes, mem, hdr, status)) return fail_all(rc);
@@ -1689,7 +1720,7 @@ static int decode_blobs_impl(cldn_decoder* d, size_t n, const void* const* blobs
     payload_bytes[f] = blob_bytes[f] - hdr[f];
     points[f] = static_cast<uint64_t>(I.width) * I.height;
     alone[f] = !route_has_frame_errors(mem, I) || I.version < 3 || points[f] > 0xFFFFFFFFull || points[f] * I.point_step > caps[f] ||
-               (mem == CLDN_MEM_HOST && payload_bytes[f] >= 10 && memcmp(payload[f], "CLOUDINI_V", 10) == 0);
+               (mem != CLDN_MEM_DEVICE && payload_bytes[f] >= 10 && memcmp(payload[f], "CLOUDINI_V", 10) == 0);
   }
   std::vector<size_t> members;
   std::vector<const void*> g_payload;

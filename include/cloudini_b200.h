@@ -14,8 +14,9 @@
  *    Pure host helpers (header, YAML, sizing, planning) work without a GPU.
  *  - Buffers are owned by the caller. `mem` says where they live: CLDN_MEM_HOST (pageable or pinned host memory;
  *    the library stages through pinned buffers and its own stream — this is the drop-in path used by
- *    cloudini_ros/src/cloudini_publisher_plugin.cpp:73-74) or CLDN_MEM_DEVICE (device pointers; launch-only,
- *    asynchronous on the handle's stream).
+ *    cloudini_ros/src/cloudini_publisher_plugin.cpp:73-74), CLDN_MEM_DEVICE (device pointers; launch-only,
+ *    asynchronous on the handle's stream) or CLDN_MEM_DEVICE_POINTS (points in device memory, blobs and payloads in
+ *    host memory: see cldn_mem_t).
  *  - Handles are not thread-safe (same as the reference's PointcloudEncoder, cloudini.hpp:185-208): one handle per
  *    thread / stream.
  */
@@ -56,7 +57,27 @@ typedef enum cldn_field_type_t {
 typedef enum cldn_encoding_opt_t { CLDN_ENC_NONE = 0, CLDN_ENC_LOSSY = 1, CLDN_ENC_LOSSLESS = 2 } cldn_encoding_opt_t;
 typedef enum cldn_compression_opt_t { CLDN_COMP_NONE = 0, CLDN_COMP_LZ4 = 1, CLDN_COMP_ZSTD = 2 } cldn_compression_opt_t;
 
-typedef enum cldn_mem_t { CLDN_MEM_HOST = 0, CLDN_MEM_DEVICE = 1 } cldn_mem_t;
+/* Where the buffers of a call live.
+ * CLDN_MEM_HOST: clouds, blobs, payloads and decoded points are host memory.
+ * CLDN_MEM_DEVICE: all of them are device memory.
+ * CLDN_MEM_DEVICE_POINTS: point clouds (encode inputs) and decoded points (decode outputs) are DEVICE pointers; blobs
+ *   and payloads (encode outputs, decode inputs) are HOST pointers. For a GPU producer or consumer of messages that
+ *   travel through host memory: only the compressed bytes cross PCIe. Accepted by cldn_b200_encode, _encode_batch,
+ *   _encode_blobs, cldn_b200_decode, _decode_batch and _decode_blobs. It takes the routes of CLDN_MEM_HOST with the
+ *   points read and written in place, so:
+ *   - every blob equals what CLDN_MEM_HOST writes for the same cloud: stage 2 runs through the system liblz4 / libzstd
+ *     (LZ4 and ZSTD blobs are the reference's bytes; ZSTD is supported);
+ *   - every decoded buffer equals what CLDN_MEM_HOST gives: only declared field bytes of the caller's device buffer are
+ *     written (padding untouched). Stage 2 is undone as for CLDN_MEM_HOST: ZSTD on the device (the system libzstd with
+ *     CLDN_B200_ZSTD_HOST=1), LZ4 by the system liblz4 on the host, then uploaded;
+ *   - statuses and messages (per frame, cldn_b200_decoder_frame_error) are those of CLDN_MEM_HOST: damaged blobs,
+ *     too-small capacities, a payload that still carries its header, a cloud that is not a whole number of points.
+ *     Nothing is written outside [0, capacity) of any buffer, host or device;
+ *   - device memory is ordered on the handle's stream only, as for CLDN_MEM_DEVICE. Encode returns when the blobs and
+ *     `written` are in host memory; decode_blobs returns with the statuses; decode / decode_batch return once the host
+ *     payloads are no longer read, and `sync` == 0 leaves the device error word to cldn_b200_decoder_sync, as for
+ *     CLDN_MEM_DEVICE. */
+typedef enum cldn_mem_t { CLDN_MEM_HOST = 0, CLDN_MEM_DEVICE = 1, CLDN_MEM_DEVICE_POINTS = 2 } cldn_mem_t;
 
 /* POD mirror of Cloudini::PointField (basic_types.hpp:50-66) */
 typedef struct cldn_field_t {
@@ -76,7 +97,8 @@ typedef struct cldn_info_t {
   uint8_t encoding_opt;    /* cldn_encoding_opt_t, default LOSSY */
   uint8_t compression_opt; /* cldn_compression_opt_t. NONE everywhere. LZ4: both APIs (device kernels; the host-pointer
                               API hands each chunk to the system liblz4). ZSTD: decode with both APIs on the device;
-                              encode through the host-pointer API only, each chunk handed to the system libzstd (dlopen) */
+                              encode with host blobs only (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS), each chunk handed to
+                              the system libzstd (dlopen) */
   uint8_t version;         /* wire version 2..5, default 5 */
   uint8_t use_threads;     /* accepted for API parity; ignored (there is no stage-2 worker thread here) */
   uint32_t n_fields;
