@@ -142,6 +142,7 @@ def lib():
     L.cldn_b200_encoder_sizes_device.argtypes = [vp]
     L.cldn_b200_encoder_sizes_device.restype = vp
     L.cldn_b200_encoder_sync.argtypes = [vp]
+    L.cldn_b200_encoder_set_stage2_on_device.argtypes = [vp, C.c_int]
     L.cldn_b200_decoder_create.argtypes = [C.c_int, vp, C.POINTER(vp)]
     L.cldn_b200_decoder_destroy.argtypes = [vp]
     L.cldn_b200_decoder_destroy.restype = None
@@ -287,6 +288,12 @@ class PointcloudEncoder:
 
     def getHeader(self) -> bytes:
         return self._header
+
+    def set_stage2_on_device(self, on: bool):
+        """Compress every LZ4 / ZSTD chunk on the device, for host and device memory alike (False: the default, the
+        system liblz4 / libzstd for host blobs, ZSTD refused for device blobs). The blobs are valid frames that the system
+        libraries and the reference decode, but not their bytes. See cldn_b200_encoder_set_stage2_on_device."""
+        _check(lib().cldn_b200_encoder_set_stage2_on_device(self._h, 1 if on else 0))
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:

@@ -277,6 +277,8 @@ const char* dev_error_text(uint32_t code) {
 struct cldn_encoder {
   cldn_info_t info;       // as given, except compression_opt = NONE (what the GPU path produces)
   int stage2 = 0;         // the caller's compression_opt (host-pointer API only)
+  bool stage2_on_device = false;  // cldn_b200_encoder_set_stage2_on_device
+  bool pooled = false;            // a handle of the per-thread pool (encoder_mark_pooled): keeps the libraries' bytes
   std::vector<uint8_t> s2_tmp;
   Plan plan;
   std::vector<uint8_t> header;
@@ -309,7 +311,7 @@ struct cldn_encoder {
   DevBuf<uint64_t> d_hash;
   DevBuf<uint8_t> d_gorilla;  // Gorilla pre-pass records: [frame][op][point][12]
   size_t last_frames = 0;
-  // stage 2 on the device (LZ4): stage-1 arena, per-chunk slots, chunk tables
+  // stage 2 on the device (LZ4, ZSTD): stage-1 arena, per-chunk (LZ4) / per-block (ZSTD) slots, chunk tables
   DevBuf<uint8_t> d_s1, d_lz_scratch;
   DevBuf<uint32_t> d_lz_chunk_frame, d_lz_chunk_sizes;
   DevBuf<Lz4Frame> d_lz_frames;
@@ -322,6 +324,10 @@ struct cldn_encoder {
 
 // LZ4_COMPRESSBOUND (lz4.h): worst case of a block for n input bytes
 static size_t lz4_bound(size_t n) { return n + n / 255 + 16; }
+
+namespace cldn {
+void encoder_mark_pooled(cldn_encoder_t* enc) { enc->pooled = true; }
+}  // namespace cldn
 
 extern "C" {
 
@@ -444,6 +450,17 @@ int cldn_b200_encoder_set_dims(cldn_encoder_t* e, uint32_t width, uint32_t heigh
   if (int rc = e->d_header.reserve(h.size())) return rc;
   CUDA_TRY(cudaMemcpy(e->d_header.p, h.data(), h.size(), cudaMemcpyHostToDevice));
   e->header = h;
+  return CLDN_OK;
+}
+
+int cldn_b200_encoder_set_stage2_on_device(cldn_encoder_t* e, int on) {
+  if (!e) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (on != 0 && on != 1) { set_error("on must be 0 or 1"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (on == 1 && e->pooled) {
+    set_error("a pool encoder (cldn_b200_pool_encoder) keeps the system libraries' stage-2 bytes: create an encoder of your own");
+    return CLDN_ERR_INVALID_ARGUMENT;
+  }
+  e->stage2_on_device = on == 1;
   return CLDN_OK;
 }
 
@@ -663,45 +680,57 @@ static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std
   return CLDN_OK;
 }
 
-// Device pointers in, device pointers out, compression LZ4: stage 1 into an internal arena, one LZ4 block per chunk on the
-// device (cldn_lz4.cu), blobs packed behind their headers. Nothing crosses PCIe except the 8-byte sizes, if asked for.
-static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
-                                   void* const* outs, const size_t* out_capacities, int write_header) {
+// Whether this encoder's stage 2 runs on the device for CLDN_MEM_DEVICE (LZ4 always, ZSTD when asked for) and for the
+// host blobs of CLDN_MEM_HOST / CLDN_MEM_DEVICE_POINTS (when asked for).
+static bool stage2_device_codec(const cldn_encoder* e, int mem) {
+  if (e->stage2 == CLDN_COMP_NONE) return false;
+  return e->stage2_on_device || (mem == CLDN_MEM_DEVICE && e->stage2 == CLDN_COMP_LZ4);
+}
+
+// Stage 1 into an internal arena, then stage 2 on the device: one LZ4 block per chunk (cldn_lz4.cu) or one ZSTD frame
+// per chunk (cldn_zstd_enc.cu), the blobs packed behind their headers into outs (device memory). The codec chooses the
+// slots and the compress launch; the arena, the chunk tables and the pack are shared. Launches: stage 1 + 2.
+static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                                      void* const* outs, const size_t* out_capacities, int write_header) {
   const cldn_info_t& info = e->info;  // compression NONE: what the stage-1 kernels produce
+  const bool zstd = e->stage2 == CLDN_COMP_ZSTD;
   cldn_info_t full = info;
-  full.compression_opt = CLDN_COMP_LZ4;
+  full.compression_opt = static_cast<uint8_t>(e->stage2);
   const size_t hdr = write_header ? e->header.size() : 0;
-  std::vector<size_t> s1_off(n_frames), s1_cap(n_frames);
-  size_t arena = 0, chunks = 0, max_chunk = 0;
+  const size_t zblock = zstd_enc_block_bytes();
+  std::vector<size_t> s1_off(n_frames), s1_cap(n_frames), blocks_per_chunk(n_frames);
+  size_t arena = 0, chunks = 0, max_chunk = 0, pieces = 0;
   for (size_t f = 0; f < n_frames; ++f) {
     size_t need;
     if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
-    const size_t n = cloud_bytes[f] / info.point_step;
+    const size_t n = cloud_bytes[f] / info.point_step, nc = (n + kChunkPoints - 1) / kChunkPoints;
     bool ok;
-    s1_cap[f] = max_compressed_size(info, n, false, &ok) + 64 * ((n + kChunkPoints - 1) / kChunkPoints + 1);
+    s1_cap[f] = max_compressed_size(info, n, false, &ok) + 64 * (nc + 1);
     s1_off[f] = arena;
     arena += (s1_cap[f] + 255) & ~size_t(255);
-    chunks += (n + kChunkPoints - 1) / kChunkPoints;
-    max_chunk = std::max(max_chunk, max_compressed_size(info, std::min<size_t>(n, kChunkPoints), false, &ok) + 64);
+    chunks += nc;
+    const size_t chunk_bound = max_compressed_size(info, std::min<size_t>(n, kChunkPoints), false, &ok) + 64;
+    max_chunk = std::max(max_chunk, chunk_bound);
+    blocks_per_chunk[f] = zstd ? std::max<size_t>(1, (chunk_bound + zblock - 1) / zblock) : 1;  // room for the worst case
+    pieces += nc * blocks_per_chunk[f];
   }
-  if (chunks > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
+  if (chunks > 0x7FFFFFFFull || pieces > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
   if (int rc = e->d_s1.reserve(arena + 256)) return rc;
-  std::vector<const void*> s1_ptr_c(n_frames);
   std::vector<void*> s1_ptr(n_frames);
   for (size_t f = 0; f < n_frames; ++f) s1_ptr[f] = e->d_s1.p + s1_off[f];
   if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, s1_ptr.data(), s1_cap.data(), 0)) return rc;
-  // chunk tables + per-chunk slots
-  const size_t slot = (lz4_bound(max_chunk) + 15) & ~size_t(15);
+  // chunk tables + slots: one per chunk (LZ4), one per block of a chunk's worst case (ZSTD)
+  const size_t slot = zstd ? zstd_enc_slot_bytes() : (lz4_bound(max_chunk) + 15) & ~size_t(15);
   if (slot > 0xFFFFFFF0ull) { set_error("chunk too large for LZ4"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = e->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
-  if (int rc = e->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
-  if (int rc = e->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
+  if (int rc = e->d_lz_scratch.reserve(std::max<size_t>(pieces, 1) * slot)) return rc;
+  if (int rc = e->d_lz_chunk_sizes.reserve(pieces + 1)) return rc;
+  if (int rc = e->d_lz_chunk_frame.reserve(2 * chunks + 2)) return rc;  // chunk -> frame, then block_begin (ZSTD)
   if (int rc = e->d_lz_frames.reserve(n_frames)) return rc;
   Lz4Frame* hf = nullptr; int hf_slot = 0;
   uint32_t* hcf = nullptr; int hcf_slot = 0;
   if (int rc = e->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
-  if (int rc = e->h_lz_chunk_frame.acquire(chunks + 1, &hcf, &hcf_slot)) return rc;
-  uint32_t cb = 0;
+  if (int rc = e->h_lz_chunk_frame.acquire(2 * chunks + 2, &hcf, &hcf_slot)) return rc;
+  uint32_t cb = 0, pb = 0;
   for (size_t f = 0; f < n_frames; ++f) {
     const size_t n = cloud_bytes[f] / info.point_step;
     Lz4Frame& F = hf[f];
@@ -712,12 +741,17 @@ static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void*
     F.blob_cap = out_capacities[f];
     F.n_chunks = static_cast<uint32_t>((n + kChunkPoints - 1) / kChunkPoints);
     F.chunk_begin = cb;
-    for (uint32_t c = 0; c < F.n_chunks; ++c) hcf[cb + c] = static_cast<uint32_t>(f);
+    for (uint32_t c = 0; c < F.n_chunks; ++c) {
+      hcf[cb + c] = static_cast<uint32_t>(f);
+      hcf[chunks + cb + c] = pb;
+      pb += static_cast<uint32_t>(blocks_per_chunk[f]);
+    }
     cb += F.n_chunks;
   }
+  hcf[2 * chunks] = pb;
   CUDA_TRY(cudaMemcpyAsync(e->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, e->stream));
   if (int rc = e->h_lz_frames.commit(hf_slot, e->stream)) return rc;
-  if (chunks) CUDA_TRY(cudaMemcpyAsync(e->d_lz_chunk_frame.p, hcf, chunks * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+  CUDA_TRY(cudaMemcpyAsync(e->d_lz_chunk_frame.p, hcf, (2 * chunks + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
   if (int rc = e->h_lz_chunk_frame.commit(hcf_slot, e->stream)) return rc;
   Lz4Launch Z{};
   Z.frames = e->d_lz_frames.p;
@@ -729,8 +763,57 @@ static int encode_batch_device_lz4(cldn_encoder* e, size_t n_frames, const void*
   Z.chunk_sizes = e->d_lz_chunk_sizes.p;
   Z.sizes = e->d_sizes.p;   // the pack kernel overwrites the stage-1 sizes with the blob sizes (it runs after every reader)
   Z.err = e->d_err.p;
-  if (launch_lz4_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) { set_error("LZ4 kernel launch failed"); return CLDN_ERR_CUDA; }
+  if (zstd) {
+    Z.block_begin = e->d_lz_chunk_frame.p + chunks;
+    Z.n_blocks_total = static_cast<uint32_t>(pieces);
+    if (launch_zstd_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  } else if (launch_lz4_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) {
+    set_error("LZ4 kernel launch failed");
+    return CLDN_ERR_CUDA;
+  }
   CUDA_TRY(cudaGetLastError());
+  return CLDN_OK;
+}
+
+// Host blobs (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS) of an encoder whose stage 2 runs on the device: the clouds go up
+// (CLDN_MEM_HOST), encode_batch_device_stage2 writes the blobs into device staging, and exactly their bytes come down.
+static int encode_batch_host_stage2(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                                    void* const* outs, const size_t* out_capacities, int write_header, size_t* written_host,
+                                    bool device_points) {
+  const size_t hdr = write_header ? e->header.size() : 0;
+  cldn_info_t full = e->info;
+  full.compression_opt = static_cast<uint8_t>(e->stage2);
+  std::vector<size_t> caps(n_frames);
+  for (size_t f = 0; f < n_frames; ++f) {
+    size_t need;
+    if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
+    // a blob never exceeds its stage-1 bytes (at most the arena's s1_cap of encode_batch_device_stage2) plus the codec's
+    // framing: stage with that much room, never more than the caller gave
+    const size_t n = cloud_bytes[f] / e->info.point_step, nc = (n + kChunkPoints - 1) / kChunkPoints;
+    bool ok;
+    const size_t s1 = max_compressed_size(e->info, n, false, &ok) + 64 * (nc + 1);
+    caps[f] = std::min(out_capacities[f], hdr + s1 + s1 / 128 + 32 * nc + 256);
+  }
+  std::vector<void*> staged, dout;
+  std::vector<const void*> din(clouds, clouds + n_frames);
+  if (!device_points) {
+    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, staged)) return rc;
+    for (size_t f = 0; f < n_frames; ++f) {
+      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(staged[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
+    }
+    din.assign(staged.begin(), staged.end());
+  }
+  if (int rc = stage_layout(e->d_out, n_frames, caps.data(), dout)) return rc;
+  if (int rc = encode_batch_device_stage2(e, n_frames, din.data(), cloud_bytes, dout.data(), caps.data(), write_header)) return rc;
+  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+  for (size_t f = 0; f < n_frames; ++f) {
+    const size_t sz = static_cast<size_t>(e->h_sizes.p[f]);
+    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], sz, cudaMemcpyDeviceToHost, e->stream));
+    if (written_host) written_host[f] = sz;
+  }
+  CUDA_TRY(cudaStreamSynchronize(e->stream));
   return CLDN_OK;
 }
 
@@ -744,12 +827,12 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   if (n_frames == 0) return CLDN_OK;
   CUDA_TRY(cudaSetDevice(e->device));
   if (mem == CLDN_MEM_DEVICE) {
-    if (e->stage2 != CLDN_COMP_NONE && e->stage2 != CLDN_COMP_LZ4) {
+    if (e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem)) {
       set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
       return CLDN_ERR_UNSUPPORTED;
     }
-    const int rc = e->stage2 == CLDN_COMP_LZ4
-                       ? encode_batch_device_lz4(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)
+    const int rc = stage2_device_codec(e, mem)
+                       ? encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)
                        : encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header);
     if (rc) return rc;
     return read_written(e, n_frames, written_host);
@@ -758,6 +841,9 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   // CLDN_MEM_DEVICE_POINTS: the host route with the clouds read in place (ordered on the handle's stream, no upload)
   const bool device_points = mem == CLDN_MEM_DEVICE_POINTS;
   const size_t hdr = write_header ? e->header.size() : 0;
+  if (stage2_device_codec(e, mem)) {
+    return encode_batch_host_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header, written_host, device_points);
+  }
   if (e->stage2 != CLDN_COMP_NONE) {
     if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
     // stage 1 on the GPU, then every chunk through the system compressor (not pipelined: this is not the product path)
@@ -872,11 +958,11 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (n_frames == 0) return CLDN_OK;
   if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
-  if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && e->stage2 != CLDN_COMP_LZ4) {
+  if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem)) {
     set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
     return CLDN_ERR_UNSUPPORTED;
   }
-  if (mem != CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
+  if (mem != CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem) && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
   cldn_info_t full = e->info;
   full.compression_opt = static_cast<uint8_t>(e->stage2);
   std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
@@ -917,8 +1003,8 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     }
     return CLDN_OK;
   }
-  const int rc = e->stage2 == CLDN_COMP_LZ4
-                     ? encode_batch_device_lz4(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0)
+  const int rc = stage2_device_codec(e, mem)
+                     ? encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0)
                      : encode_batch_device(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0);
   if (rc) return rc;
   const size_t tab_bytes = (2 * n_frames + 1) * sizeof(uint64_t) + headers.size();

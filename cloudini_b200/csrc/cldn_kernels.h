@@ -166,8 +166,17 @@ struct Lz4Launch {
   uint64_t* sizes;             // per frame: bytes written by the pack kernel (0: did not fit)
   uint32_t* err;
   uint32_t* frame_err;         // decompression: nullptr, or one word per frame (see frame_err_word)
+  // ZSTD compression: a chunk's compressed bytes are the concatenation of several pieces (one per block). Chunk gc owns
+  // pieces block_begin[gc] .. block_begin[gc + 1] - 1, and the slots of `scratch` and `chunk_sizes` are per piece.
+  // nullptr: one piece per chunk (LZ4).
+  const uint32_t* block_begin = nullptr;  // n_chunks_total + 1 entries
+  uint32_t n_blocks_total = 0;
 };
+// Compression: one LZ4 block per chunk, then the blobs are packed (launch_stage2_pack)
 int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
+// Blob f = header + ([u32 size][the chunk's pieces])* into F.blob_out; a blob that does not fit F.blob_cap raises
+// DEV_ERR_ENCODE_OUTPUT_SMALL and writes sizes[f] = 0, else sizes[f] = its bytes.
+int launch_stage2_pack(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
 int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream);
 // Re-frames the slots of L (chunk_sizes[] bytes each) into one stage-1 payload per frame at plain_out; a payload that
 // does not fit plain_cap raises `fail_code`.
@@ -184,6 +193,12 @@ struct ZstdLaunch {
   uint8_t* lit_scratch;    // n_ctas * zstd_warps_per_cta() regions of zstd_lit_scratch_bytes(body_cap) bytes
 };
 uint32_t zstd_warps_per_cta();
+// ---- ZSTD compression on the device (cldn_zstd_enc.cu) -----------------------------------------------------------------
+// Every chunk of L becomes one ZSTD frame of Huffman-coded literal blocks of zstd_enc_block_bytes() stage-1 bytes (the
+// pieces of L.block_begin, zstd_enc_slot_bytes() each), then the blobs are packed (launch_stage2_pack).
+uint32_t zstd_enc_block_bytes();
+uint32_t zstd_enc_slot_bytes();
+int launch_zstd_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
 size_t zstd_lit_scratch_bytes(uint32_t body_cap);
 int launch_zstd_decompress(const ZstdLaunch& Z, cudaStream_t stream);
 

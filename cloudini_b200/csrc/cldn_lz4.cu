@@ -242,7 +242,8 @@ __global__ void __launch_bounds__(kLzThreads) lz4_decompress_chunks_kernel(const
 }
 
 // One CTA per frame: ([u32 size][bytes])* of the frame's chunks, back to back at `dst` (behind `header_bytes` bytes of
-// header, which are copied too); the frame's total goes to sizes[f]. Stores are checked against dst_cap.
+// header, which are copied too); the frame's total goes to sizes[f]. Stores are checked against dst_cap. A chunk's bytes
+// are its slot, or with L.block_begin the concatenation of its pieces (ZSTD compression).
 // (shared by the ZSTD decompressor, launch_stage2_unpack: `unpack_err` is the code of a re-framed payload that does not fit)
 __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L, const uint8_t* header, uint32_t header_bytes, int to_blob,
                                                               uint32_t unpack_err) {
@@ -258,12 +259,17 @@ __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L,
   bool fits = header_bytes <= cap;
   for (uint32_t c = 0; c < F.n_chunks; ++c) {
     const uint32_t gc = F.chunk_begin + c;
-    const uint32_t sz = L.chunk_sizes[gc];
-    const uint8_t* src = L.scratch + static_cast<size_t>(gc) * L.slot_stride;
+    const uint32_t p0 = L.block_begin ? L.block_begin[gc] : gc, p1 = L.block_begin ? L.block_begin[gc + 1] : gc + 1;
+    uint64_t sz = 0;
+    for (uint32_t p = p0; p < p1; ++p) sz += L.chunk_sizes[p];
     if (pos + 4ull + sz > cap) { fits = false; break; }
-    if (threadIdx.x == 0) store_u32(dst + pos, sz);
-    lz_copy(dst + pos + 4u, src, sz, threadIdx.x, blockDim.x);
-    pos += 4ull + sz;
+    if (threadIdx.x == 0) store_u32(dst + pos, static_cast<uint32_t>(sz));
+    pos += 4ull;
+    for (uint32_t p = p0; p < p1; ++p) {
+      const uint32_t psz = L.chunk_sizes[p];
+      lz_copy(dst + pos, L.scratch + static_cast<size_t>(p) * L.slot_stride, psz, threadIdx.x, blockDim.x);
+      pos += psz;
+    }
   }
   if (threadIdx.x == 0) {
     s_pos = pos;
@@ -273,16 +279,22 @@ __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L,
   (void)s_pos;
 }
 
+int launch_stage2_pack(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream) {
+  if (L.n_frames == 0) return 0;
+  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, header, header_bytes, 1, DEV_ERR_LZ4);
+  count_launch(1);
+  return 1;
+}
+
 int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream) {
   if (L.n_frames == 0) return 0;
   int n = 0;
   if (L.n_chunks_total) {
     lz4_compress_chunks_kernel<<<(L.n_chunks_total + kLzWarps - 1) / kLzWarps, kLzThreads, 0, stream>>>(L);
+    count_launch(1);
     ++n;
   }
-  lz4_pack_frames_kernel<<<L.n_frames, 256, 0, stream>>>(L, header, header_bytes, 1, DEV_ERR_LZ4);
-  count_launch(n + 1);
-  return n + 1;
+  return n + launch_stage2_pack(L, header, header_bytes, stream);
 }
 
 int launch_lz4_decompress(const Lz4Launch& L, cudaStream_t stream) {

@@ -80,6 +80,9 @@ size_t leading_lossy_float_count(const cldn_info_t& info);
 size_t max_serialized_field_size(const cldn_field_t& f, uint8_t encoding_opt, bool* ok);
 
 void set_error(const char* fmt, ...);
+// Marks an encoder as one of the per-thread pool's (cldn_ros.cpp): the converter and the shims hand it to callers that
+// were promised the system libraries' bytes, so it refuses cldn_b200_encoder_set_stage2_on_device(enc, 1).
+void encoder_mark_pooled(cldn_encoder_t* enc);
 int size_of_type(uint8_t type);
 
 }  // namespace cldn

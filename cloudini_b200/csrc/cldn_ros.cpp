@@ -325,6 +325,7 @@ struct HandlePool {
     if (!ready()) { set_error("cudaStreamCreate failed"); return nullptr; }
     cldn_encoder_t* enc = nullptr;
     if (cldn_b200_encoder_create(&info, -1, stream, &enc) != CLDN_OK) return nullptr;
+    cldn::encoder_mark_pooled(enc);  // the converter and the shims promise the system libraries' bytes
     LayoutKey k;
     k.info = info;
     encoders.insert(encoders.begin(), {k, enc});

@@ -97,8 +97,9 @@ typedef struct cldn_info_t {
   uint8_t encoding_opt;    /* cldn_encoding_opt_t, default LOSSY */
   uint8_t compression_opt; /* cldn_compression_opt_t. NONE everywhere. LZ4: both APIs (device kernels; the host-pointer
                               API hands each chunk to the system liblz4). ZSTD: decode with both APIs on the device;
-                              encode with host blobs only (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS), each chunk handed to
-                              the system libzstd (dlopen) */
+                              encode with host blobs (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS), each chunk handed to the
+                              system libzstd (dlopen), and with every memory kind on the device for an encoder given
+                              cldn_b200_encoder_set_stage2_on_device(enc, 1) */
   uint8_t version;         /* wire version 2..5, default 5 */
   uint8_t use_threads;     /* accepted for API parity; ignored (there is no stage-2 worker thread here) */
   uint32_t n_fields;
@@ -191,6 +192,16 @@ const uint64_t* cldn_b200_encoder_sizes_device(const cldn_encoder_t* enc);
  * reference constructs a PointcloudEncoder per message, ros_msg_utils.cpp:198, which here would mean streams, device
  * buffers and pinned memory per message). Only the header text changes. Synchronises the handle's stream. */
 int cldn_b200_encoder_set_dims(cldn_encoder_t* enc, uint32_t width, uint32_t height);
+/* Where this encoder's LZ4 / ZSTD stage 2 runs. 0 (default): as before. LZ4 runs on the device for CLDN_MEM_DEVICE and in
+ * the system liblz4 for host blobs. ZSTD runs in the system libzstd for host blobs and is refused for CLDN_MEM_DEVICE.
+ * 1: every LZ4 / ZSTD chunk is compressed on the device, for all three memory kinds. Blobs are valid frames that
+ * libzstd / liblz4 and the reference decode to the same stage-1 bytes, but they are not the system libraries' bytes.
+ * A blob's bytes do not depend on the memory kind, the call (encode, encode_batch, encode_blobs; headers aside), the
+ * other frames of the batch or the stream. Capacities, statuses and messages are those of the default; NONE is
+ * unaffected. The header, dims and cldn_b200_encoder_info are untouched. Returns CLDN_ERR_INVALID_ARGUMENT for an `on`
+ * other than 0 or 1, and for on = 1 on a handle of the per-thread pool (cldn_b200_pool_encoder), which the DDS converter
+ * and the ros shims share and which keeps the system libraries' bytes. */
+int cldn_b200_encoder_set_stage2_on_device(cldn_encoder_t* enc, int on);
 /* Waits for everything enqueued on the handle's stream; reports device-side errors of the last call. */
 int cldn_b200_encoder_sync(cldn_encoder_t* enc);
 

@@ -111,7 +111,9 @@ int cldn_b200_ros_convert_msg(const void* dds_msg, size_t msg_bytes, const char*
 /* Handles of the calling thread's pool (created on first use, owned by the library, never to be destroyed by the caller;
  * valid for this thread only). The reference constructs encoder / decoder objects per message, which costs it nothing;
  * a GPU handle owns streams, device buffers and pinned memory, so the per-message callers (the shims of
- * convertPointCloud2ToCompressedCloud & co.) take theirs from here. The encoder is re-dimensioned to info->width / height. */
+ * convertPointCloud2ToCompressedCloud & co.) take theirs from here. The encoder is re-dimensioned to info->width / height.
+ * It keeps the system libraries' stage-2 bytes: cldn_b200_encoder_set_stage2_on_device(enc, 1) refuses it
+ * (CLDN_ERR_INVALID_ARGUMENT). cldn_b200_ros_compress_msg uses the handle it is given, with that handle's policy. */
 int cldn_b200_pool_encoder(const cldn_info_t* info, cldn_encoder_t** out);
 int cldn_b200_pool_decoder(cldn_decoder_t** out);
 int cldn_b200_pool_preproc(cldn_preproc_t** out);
