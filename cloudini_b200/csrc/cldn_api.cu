@@ -276,7 +276,8 @@ const char* dev_error_text(uint32_t code) {
 // =====================================================================================================================
 struct cldn_encoder {
   cldn_info_t info;       // as given, except compression_opt = NONE (what the GPU path produces)
-  int stage2 = 0;         // the caller's compression_opt (host-pointer API only)
+  cldn_info_t blob_info;  // the blob's layout: as given, compression_opt as declared
+  int stage2 = 0;         // the caller's compression_opt
   bool stage2_on_device = false;  // cldn_b200_encoder_set_stage2_on_device
   bool pooled = false;            // a handle of the per-thread pool (encoder_mark_pooled): keeps the libraries' bytes
   std::vector<uint8_t> s2_tmp;
@@ -310,7 +311,6 @@ struct cldn_encoder {
   PinRing<uint32_t> h_chunk_frame;
   DevBuf<uint64_t> d_hash;
   DevBuf<uint8_t> d_gorilla;  // Gorilla pre-pass records: [frame][op][point][12]
-  size_t last_frames = 0;
   // stage 2 on the device (LZ4, ZSTD): stage-1 arena, per-chunk (LZ4) / per-block (ZSTD) slots, chunk tables
   DevBuf<uint8_t> d_s1, d_lz_scratch;
   DevBuf<uint32_t> d_lz_chunk_frame, d_lz_chunk_sizes;
@@ -328,6 +328,18 @@ static size_t lz4_bound(size_t n) { return n + n / 255 + 16; }
 namespace cldn {
 void encoder_mark_pooled(cldn_encoder_t* enc) { enc->pooled = true; }
 }  // namespace cldn
+
+static int check_device_error(cudaStream_t stream, uint32_t* d_err, uint32_t* h_err) {
+  CUDA_TRY(cudaMemcpyAsync(h_err, d_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  CUDA_TRY(cudaStreamSynchronize(stream));
+  if (*h_err != DEV_OK) {
+    const uint32_t code = *h_err;
+    cudaMemsetAsync(d_err, 0, sizeof(uint32_t), stream);
+    set_error("%s", dev_error_text(code));
+    return code == DEV_ERR_ENCODE_OUTPUT_SMALL ? CLDN_ERR_BUFFER_TOO_SMALL : CLDN_ERR_CORRUPT_DATA;
+  }
+  return CLDN_OK;
+}
 
 extern "C" {
 
@@ -381,6 +393,7 @@ int cldn_b200_encoder_create(const cldn_info_t* info, int device, void* stream, 
   if (int rc = select_device(device)) return rc;
   cldn_encoder* e = new cldn_encoder();
   e->info = *info;
+  e->blob_info = *info;
   e->stage2 = info->compression_opt;        // the header declares it; the kernels always produce stage 1
   e->info.compression_opt = CLDN_COMP_NONE;
   e->plan = plan;
@@ -429,8 +442,7 @@ int cldn_b200_encoder_header(const cldn_encoder_t* enc, const uint8_t** header, 
 
 int cldn_b200_encoder_info(const cldn_encoder_t* enc, cldn_info_t* info) {
   if (!enc || !info) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
-  *info = enc->info;
-  info->compression_opt = static_cast<uint8_t>(enc->stage2);  // as the caller gave it
+  *info = enc->blob_info;
   return CLDN_OK;
 }
 
@@ -440,11 +452,9 @@ int cldn_b200_encoder_set_dims(cldn_encoder_t* e, uint32_t width, uint32_t heigh
   if (!e) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (e->info.width == width && e->info.height == height) return CLDN_OK;
   CUDA_TRY(cudaSetDevice(e->device));
-  e->info.width = width;
-  e->info.height = height;
-  cldn_info_t full = e->info;
-  full.compression_opt = static_cast<uint8_t>(e->stage2);
-  const std::vector<uint8_t> h = make_header(full);
+  e->info.width = e->blob_info.width = width;
+  e->info.height = e->blob_info.height = height;
+  const std::vector<uint8_t> h = make_header(e->blob_info);
   // the device copy of the previous header may still be read by kernels in flight on the handle's stream
   CUDA_TRY(cudaStreamSynchronize(e->stream));
   if (int rc = e->d_header.reserve(h.size())) return rc;
@@ -464,29 +474,133 @@ int cldn_b200_encoder_set_stage2_on_device(cldn_encoder_t* e, int on) {
   return CLDN_OK;
 }
 
-static int check_device_error(cudaStream_t stream, uint32_t* d_err, uint32_t* h_err) {
-  CUDA_TRY(cudaMemcpyAsync(h_err, d_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-  CUDA_TRY(cudaStreamSynchronize(stream));
-  if (*h_err != DEV_OK) {
-    const uint32_t code = *h_err;
-    cudaMemsetAsync(d_err, 0, sizeof(uint32_t), stream);
-    set_error("%s", dev_error_text(code));
-    return code == DEV_ERR_ENCODE_OUTPUT_SMALL ? CLDN_ERR_BUFFER_TOO_SMALL : CLDN_ERR_CORRUPT_DATA;
-  }
-  return CLDN_OK;
-}
-
 int cldn_b200_encoder_sync(cldn_encoder_t* e) {
   if (!e) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
   CUDA_TRY(cudaSetDevice(e->device));
   return check_device_error(e->stream, e->d_err.p, e->h_err.p);
 }
 
-// Enqueues the kernels for a batch whose inputs/outputs are device pointers.
+}  // extern "C"
+
+// No C++ exception may cross the C ABI (std::terminate under ctypes / C callers): allocation failures become a status.
+template <class Fn>
+static int guarded(Fn&& fn) {
+  try {
+    return fn();
+  } catch (const std::bad_alloc&) {
+    set_error("out of memory");
+    return CLDN_ERR_INTERNAL;
+  } catch (const std::exception& ex) {
+    set_error("internal error: %s", ex.what());
+    return CLDN_ERR_INTERNAL;
+  }
+}
+
+// The encoder's rules for one frame, which every entry point checks on all frames before it uploads or launches
+// anything: the reference's checks in its order (cloudini.cpp:523-534), then this library's own. `hdr` is the header
+// bytes written in front of the payload at `out`.
+static int check_encode_frame(const cldn_encoder* e, size_t hdr, const void* cloud, size_t cloud_bytes, const void* out,
+                              size_t out_capacity) {
+  const cldn_info_t& blob = e->blob_info;
+  if (blob.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (cloud_bytes % blob.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
+  const size_t n = cloud_bytes / blob.point_step;
+  bool ok;
+  const size_t need = max_compressed_size(blob, n, false, &ok) + hdr;
+  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
+  if (out_capacity < need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
+  if (n > 0xFFFFFFFFull) { set_error("too many points in one frame"); return CLDN_ERR_UNSUPPORTED; }
+  if ((n > 0 && !cloud) || (need > 0 && !out)) { set_error("null frame pointer"); return CLDN_ERR_INVALID_ARGUMENT; }
+  return CLDN_OK;
+}
+
+// How a batch is encoded. Device routes write CLDN_MEM_DEVICE blobs; host routes write host blobs from host clouds
+// (CLDN_MEM_HOST) or device clouds (CLDN_MEM_DEVICE_POINTS).
+enum EncodeRoute {
+  kEncDevice,        // stage 1
+  kEncDeviceStage2,  // stage 1, then LZ4 / ZSTD on the device
+  kEncHostPlain,     // stage 1, pipelined upload / encode / download
+  kEncHostStage2,    // stage 1 and LZ4 / ZSTD on the device, then download
+  kEncHostLibrary,   // stage 1, download, then liblz4 / libzstd on the host
+};
+
+// The route for this encoder and memory kind, or the refusal. LZ4 runs on the device for device blobs; ZSTD, and LZ4
+// into host blobs, run on the device only when the caller asked for it (cldn_b200_encoder_set_stage2_on_device).
+static int choose_encode_route(const cldn_encoder* e, int mem, EncodeRoute* route) {
+  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
+  const bool device_blobs = mem == CLDN_MEM_DEVICE;
+  if (e->stage2 == CLDN_COMP_NONE) {
+    *route = device_blobs ? kEncDevice : kEncHostPlain;
+  } else if (e->stage2_on_device || (device_blobs && e->stage2 == CLDN_COMP_LZ4)) {
+    *route = device_blobs ? kEncDeviceStage2 : kEncHostStage2;
+  } else if (device_blobs) {
+    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
+    return CLDN_ERR_UNSUPPORTED;
+  } else {
+    if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
+    *route = kEncHostLibrary;
+  }
+  return CLDN_OK;
+}
+
+// The internal stage-1 arena of the compressed routes for a frame of n points: the stage-1 worst case plus 64 bytes per
+// chunk and 64 more.
+static size_t stage1_arena_bytes(const cldn_encoder* e, size_t n) {
+  bool ok;
+  return max_compressed_size(e->info, n, false, &ok) + 64 * ((n + kChunkPoints - 1) / kChunkPoints + 1);
+}
+
+// Device staging of a plain host blob. A committed V5 mode can exceed the reference's own worst-case formula (DeltaRle on
+// a 64-bit field: 11 bytes per value against the 10 it budgets); the reference then succeeds iff the caller's buffer is
+// large enough. Stage with room for the real worst case, never more than the caller gave: the kernels check every store
+// against this bound.
+static size_t plain_blob_staging(const cldn_encoder* e, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
+  const size_t n = cloud_bytes / e->info.point_step;
+  bool ok;
+  size_t worst = max_compressed_size(e->info, n, false, &ok) + hdr;
+  for (uint32_t s = 0; s < e->plan.n_sections; ++s) {
+    if (e->plan.sections[s].bpv == 8) worst += n + 16 * (n / kChunkPoints + 1);
+  }
+  return std::min(out_capacity, worst);
+}
+
+// Device staging of a host blob whose stage 2 runs on the device: a blob never exceeds its stage-1 arena plus the codec's
+// framing. Never more than the caller gave.
+static size_t stage2_blob_staging(const cldn_encoder* e, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
+  const size_t n = cloud_bytes / e->info.point_step, s1 = stage1_arena_bytes(e, n);
+  return std::min(out_capacity, hdr + s1 + s1 / 128 + 32 * ((n + kChunkPoints - 1) / kChunkPoints) + 256);
+}
+
+// Device-pointer batches: the blob sizes into written_host, if asked for (one read-back, synchronises).
+static int read_written(cldn_encoder* e, size_t n_frames, size_t* written_host) {
+  if (!written_host) return CLDN_OK;
+  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+  for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
+  return CLDN_OK;
+}
+
+// Staging: n byte ranges at 256-byte-aligned offsets of `buf`, which grows to hold them with 256 bytes to
+// spare; at[f] is where range f starts.
+static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std::vector<void*>& at) {
+  std::vector<size_t> off(n);
+  size_t total = 0;
+  for (size_t f = 0; f < n; ++f) {
+    off[f] = total;
+    total += (bytes[f] + 255) & ~size_t(255);
+  }
+  if (int rc = buf.reserve(total + 256)) return rc;
+  at.resize(n);
+  for (size_t f = 0; f < n; ++f) at[f] = buf.p + off[f];
+  return CLDN_OK;
+}
+
+// Stage 1 of frames that passed check_encode_frame, or of staging their caller sized: fills their EncFrames and enqueues
+// the kernels. Inputs and outputs are device pointers; the kernels check every store against out_capacities.
 static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                                void* const* outs, const size_t* out_capacities, int write_header) {
   const cldn_info_t& info = e->info;
-  if (info.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }  // cloudini.cpp:523-525
   EncFrame* hf = nullptr;
   int hf_slot = 0;
   if (int rc = e->h_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
@@ -497,20 +611,7 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
   uint64_t tiles = 0, chunks = 0;
   bool aligned16 = true;
   for (size_t f = 0; f < n_frames; ++f) {
-    if (cloud_bytes[f] % info.point_step != 0) {
-      set_error("Input cloud_data size is not a multiple of point_step");  // cloudini.cpp:526-528
-      return CLDN_ERR_INVALID_ARGUMENT;
-    }
     const size_t n = cloud_bytes[f] / info.point_step;
-    if (n > 0xFFFFFFFFull) { set_error("too many points in one frame"); return CLDN_ERR_UNSUPPORTED; }
-    bool ok;
-    const size_t need = max_compressed_size(info, n, false, &ok) + hdr;  // cloudini.cpp:530-534
-    if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-    if (out_capacities[f] < need) {
-      set_error("Output buffer too small for worst-case compressed size");
-      return CLDN_ERR_BUFFER_TOO_SMALL;
-    }
-    if (n > 0 && (!clouds[f] || !outs[f])) { set_error("null frame pointer"); return CLDN_ERR_INVALID_ARGUMENT; }
     EncFrame& F = hf[f];
     F.in = static_cast<const uint8_t*>(clouds[f]);
     F.out = static_cast<uint8_t*>(outs[f]);
@@ -623,68 +724,7 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
     if (launch_encode_regular(e->plan, L, e->stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
   }
   CUDA_TRY(cudaGetLastError());
-  e->last_frames = n_frames;
   return CLDN_OK;
-}
-
-}  // extern "C"
-
-// No C++ exception may cross the C ABI (std::terminate under ctypes / C callers): allocation failures become a status.
-template <class Fn>
-static int guarded(Fn&& fn) {
-  try {
-    return fn();
-  } catch (const std::bad_alloc&) {
-    set_error("out of memory");
-    return CLDN_ERR_INTERNAL;
-  } catch (const std::exception& ex) {
-    set_error("internal error: %s", ex.what());
-    return CLDN_ERR_INTERNAL;
-  }
-}
-
-// The reference's checks of one frame to encode, in its order (cloudini.cpp:523-534). `full` is the layout with the
-// compression the blob declares and `hdr` the header bytes written in front; *need is the worst-case blob size.
-static int check_encode_frame(const cldn_info_t& full, size_t hdr, size_t cloud_bytes, size_t out_capacity, size_t* need) {
-  if (full.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
-  if (cloud_bytes % full.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
-  bool ok;
-  *need = max_compressed_size(full, cloud_bytes / full.point_step, false, &ok) + hdr;
-  if (!ok) return CLDN_ERR_INVALID_ARGUMENT;
-  if (out_capacity < *need) { set_error("Output buffer too small for worst-case compressed size"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-  return CLDN_OK;
-}
-
-// Device-pointer batches: the blob sizes into written_host, if asked for (one read-back, synchronises).
-static int read_written(cldn_encoder* e, size_t n_frames, size_t* written_host) {
-  if (!written_host) return CLDN_OK;
-  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
-  return CLDN_OK;
-}
-
-// Host-pointer staging: n byte ranges at 256-byte-aligned offsets of `buf`, which grows to hold them with 256 bytes to
-// spare; at[f] is where range f starts.
-static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std::vector<void*>& at) {
-  std::vector<size_t> off(n);
-  size_t total = 0;
-  for (size_t f = 0; f < n; ++f) {
-    off[f] = total;
-    total += (bytes[f] + 255) & ~size_t(255);
-  }
-  if (int rc = buf.reserve(total + 256)) return rc;
-  at.resize(n);
-  for (size_t f = 0; f < n; ++f) at[f] = buf.p + off[f];
-  return CLDN_OK;
-}
-
-// Whether this encoder's stage 2 runs on the device for CLDN_MEM_DEVICE (LZ4 always, ZSTD when asked for) and for the
-// host blobs of CLDN_MEM_HOST / CLDN_MEM_DEVICE_POINTS (when asked for).
-static bool stage2_device_codec(const cldn_encoder* e, int mem) {
-  if (e->stage2 == CLDN_COMP_NONE) return false;
-  return e->stage2_on_device || (mem == CLDN_MEM_DEVICE && e->stage2 == CLDN_COMP_LZ4);
 }
 
 // Stage 1 into an internal arena, then stage 2 on the device: one LZ4 block per chunk (cldn_lz4.cu) or one ZSTD frame
@@ -694,30 +734,23 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
                                       void* const* outs, const size_t* out_capacities, int write_header) {
   const cldn_info_t& info = e->info;  // compression NONE: what the stage-1 kernels produce
   const bool zstd = e->stage2 == CLDN_COMP_ZSTD;
-  cldn_info_t full = info;
-  full.compression_opt = static_cast<uint8_t>(e->stage2);
   const size_t hdr = write_header ? e->header.size() : 0;
   const size_t zblock = zstd_enc_block_bytes();
-  std::vector<size_t> s1_off(n_frames), s1_cap(n_frames), blocks_per_chunk(n_frames);
-  size_t arena = 0, chunks = 0, max_chunk = 0, pieces = 0;
+  std::vector<size_t> s1_cap(n_frames), blocks_per_chunk(n_frames);
+  size_t chunks = 0, max_chunk = 0, pieces = 0;
   for (size_t f = 0; f < n_frames; ++f) {
-    size_t need;
-    if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
     const size_t n = cloud_bytes[f] / info.point_step, nc = (n + kChunkPoints - 1) / kChunkPoints;
-    bool ok;
-    s1_cap[f] = max_compressed_size(info, n, false, &ok) + 64 * (nc + 1);
-    s1_off[f] = arena;
-    arena += (s1_cap[f] + 255) & ~size_t(255);
+    s1_cap[f] = stage1_arena_bytes(e, n);
     chunks += nc;
+    bool ok;
     const size_t chunk_bound = max_compressed_size(info, std::min<size_t>(n, kChunkPoints), false, &ok) + 64;
     max_chunk = std::max(max_chunk, chunk_bound);
     blocks_per_chunk[f] = zstd ? std::max<size_t>(1, (chunk_bound + zblock - 1) / zblock) : 1;  // room for the worst case
     pieces += nc * blocks_per_chunk[f];
   }
   if (chunks > 0x7FFFFFFFull || pieces > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = e->d_s1.reserve(arena + 256)) return rc;
-  std::vector<void*> s1_ptr(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) s1_ptr[f] = e->d_s1.p + s1_off[f];
+  std::vector<void*> s1_ptr;
+  if (int rc = stage_layout(e->d_s1, n_frames, s1_cap.data(), s1_ptr)) return rc;
   if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, s1_ptr.data(), s1_cap.data(), 0)) return rc;
   // chunk tables + slots: one per chunk (LZ4), one per block of a chunk's worst case (ZSTD)
   const size_t slot = zstd ? zstd_enc_slot_bytes() : (lz4_bound(max_chunk) + 15) & ~size_t(15);
@@ -735,7 +768,7 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
     const size_t n = cloud_bytes[f] / info.point_step;
     Lz4Frame& F = hf[f];
     memset(&F, 0, sizeof(F));
-    F.plain = e->d_s1.p + s1_off[f];
+    F.plain = static_cast<uint8_t*>(s1_ptr[f]);
     F.plain_bytes = e->d_sizes.p + f;
     F.blob_out = static_cast<uint8_t*>(outs[f]);
     F.blob_cap = out_capacities[f];
@@ -775,146 +808,41 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
   return CLDN_OK;
 }
 
-// Host blobs (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS) of an encoder whose stage 2 runs on the device: the clouds go up
-// (CLDN_MEM_HOST), encode_batch_device_stage2 writes the blobs into device staging, and exactly their bytes come down.
-static int encode_batch_host_stage2(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
-                                    void* const* outs, const size_t* out_capacities, int write_header, size_t* written_host,
-                                    bool device_points) {
-  const size_t hdr = write_header ? e->header.size() : 0;
-  cldn_info_t full = e->info;
-  full.compression_opt = static_cast<uint8_t>(e->stage2);
-  std::vector<size_t> caps(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) {
-    size_t need;
-    if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
-    // a blob never exceeds its stage-1 bytes (at most the arena's s1_cap of encode_batch_device_stage2) plus the codec's
-    // framing: stage with that much room, never more than the caller gave
-    const size_t n = cloud_bytes[f] / e->info.point_step, nc = (n + kChunkPoints - 1) / kChunkPoints;
-    bool ok;
-    const size_t s1 = max_compressed_size(e->info, n, false, &ok) + 64 * (nc + 1);
-    caps[f] = std::min(out_capacities[f], hdr + s1 + s1 / 128 + 32 * nc + 256);
-  }
-  std::vector<void*> staged, dout;
+// Host blobs (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS) through device staging bounded by caps[f]: the clouds go up on the
+// h2d stream (CLDN_MEM_HOST), the blobs are encoded on the handle's stream, and once a blob's 8-byte size is back,
+// exactly that many bytes come down on the d2h stream. Stage 1 alone is pipelined frame by frame: frame f is encoded
+// while later frames go up and earlier ones come down. Device stage 2 encodes the batch at once and is checked before
+// anything comes down.
+static int encode_host_blobs(cldn_encoder* e, bool device_stage2, size_t n_frames, const void* const* clouds,
+                             const size_t* cloud_bytes, void* const* outs, const size_t* caps, int write_header,
+                             size_t* written_host, bool device_points) {
+  std::vector<void*> slots, dout;
   std::vector<const void*> din(clouds, clouds + n_frames);
   if (!device_points) {
-    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, staged)) return rc;
-    for (size_t f = 0; f < n_frames; ++f) {
-      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(staged[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
-    }
-    din.assign(staged.begin(), staged.end());
+    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, slots)) return rc;
   }
-  if (int rc = stage_layout(e->d_out, n_frames, caps.data(), dout)) return rc;
-  if (int rc = encode_batch_device_stage2(e, n_frames, din.data(), cloud_bytes, dout.data(), caps.data(), write_header)) return rc;
-  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) {
-    const size_t sz = static_cast<size_t>(e->h_sizes.p[f]);
-    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], sz, cudaMemcpyDeviceToHost, e->stream));
-    if (written_host) written_host[f] = sz;
-  }
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return CLDN_OK;
-}
-
-static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
-                             void* const* outs, const size_t* out_capacities, int write_header, size_t* written_host,
-                             int mem) {
-  if (!e || (n_frames && (!clouds || !cloud_bytes || !outs || !out_capacities))) {
-    set_error("null argument");
-    return CLDN_ERR_INVALID_ARGUMENT;
-  }
-  if (n_frames == 0) return CLDN_OK;
-  CUDA_TRY(cudaSetDevice(e->device));
-  if (mem == CLDN_MEM_DEVICE) {
-    if (e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem)) {
-      set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
-      return CLDN_ERR_UNSUPPORTED;
-    }
-    const int rc = stage2_device_codec(e, mem)
-                       ? encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)
-                       : encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header);
-    if (rc) return rc;
-    return read_written(e, n_frames, written_host);
-  }
-  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
-  // CLDN_MEM_DEVICE_POINTS: the host route with the clouds read in place (ordered on the handle's stream, no upload)
-  const bool device_points = mem == CLDN_MEM_DEVICE_POINTS;
-  const size_t hdr = write_header ? e->header.size() : 0;
-  if (stage2_device_codec(e, mem)) {
-    return encode_batch_host_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header, written_host, device_points);
-  }
-  if (e->stage2 != CLDN_COMP_NONE) {
-    if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
-    // stage 1 on the GPU, then every chunk through the system compressor (not pipelined: this is not the product path)
-    cldn_info_t full = e->info;
-    full.compression_opt = static_cast<uint8_t>(e->stage2);
-    for (size_t f = 0; f < n_frames; ++f) {
-      size_t need;
-      if (int rc = check_encode_frame(full, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
-      bool ok;
-      size_t cap1 = max_compressed_size(e->info, cloud_bytes[f] / e->info.point_step, false, &ok);
-      if (int rc = e->d_out.reserve(cap1 + 256)) return rc;
-      const void* din = clouds[f];
-      if (!device_points) {
-        if (int rc = e->d_in.reserve(cloud_bytes[f] + 256)) return rc;
-        if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(e->d_in.p, clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->stream));
-        din = e->d_in.p;
-      }
-      void* dout = e->d_out.p;
-      if (int rc = encode_batch_device(e, 1, &din, &cloud_bytes[f], &dout, &cap1, 0)) return rc;
-      if (int rc = e->h_sizes.reserve(1)) return rc;
-      CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-      if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-      const size_t s1 = static_cast<size_t>(e->h_sizes.p[0]);
-      if (s1 > cap1) { set_error("Output buffer too small for uncompressed chunk"); return CLDN_ERR_BUFFER_TOO_SMALL; }
-      e->s2_tmp.resize(s1 + 16);
-      if (s1) CUDA_TRY(cudaMemcpy(e->s2_tmp.data(), e->d_out.p, s1, cudaMemcpyDeviceToHost));
-      uint8_t* out = static_cast<uint8_t*>(outs[f]);
-      if (hdr) memcpy(out, e->header.data(), hdr);
-      size_t w = 0;
-      if (int rc = stage2_compress_payload(e->stage2, e->s2_tmp.data(), s1, out + hdr, out_capacities[f] - hdr, &w)) return rc;
-      if (written_host) written_host[f] = hdr + w;
-    }
-    return CLDN_OK;
-  }
-  // ---- host path: H2D -> kernels -> D2H (sizes first, then exactly the encoded bytes) ----
-  std::vector<size_t> caps(n_frames);
-  for (size_t f = 0; f < n_frames; ++f) {
-    size_t need;
-    if (int rc = check_encode_frame(e->info, hdr, cloud_bytes[f], out_capacities[f], &need)) return rc;
-    // A committed V5 mode can exceed the reference's own worst-case formula (DeltaRle on a 64-bit field: 11 bytes per
-    // value against the 10 it budgets); the reference then succeeds iff the caller's buffer is large enough. Stage with
-    // room for the real worst case, never more than the caller gave: the kernels check every store against this bound.
-    size_t worst = need;
-    for (uint32_t s2 = 0; s2 < e->plan.n_sections; ++s2) {
-      if (e->plan.sections[s2].bpv == 8) worst += cloud_bytes[f] / e->info.point_step + 16 * ((cloud_bytes[f] / e->info.point_step) / kChunkPoints + 1);
-    }
-    caps[f] = std::min(out_capacities[f], worst);
-  }
-  std::vector<void*> staged, dout;
-  std::vector<const void*> din(clouds, clouds + n_frames);
-  if (!device_points) {
-    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, staged)) return rc;
-    din.assign(staged.begin(), staged.end());
-  }
-  if (int rc = stage_layout(e->d_out, n_frames, caps.data(), dout)) return rc;
+  if (int rc = stage_layout(e->d_out, n_frames, caps, dout)) return rc;
   if (int rc = e->pipe.ensure(2 * n_frames)) return rc;
   if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-  // frame f: upload on the h2d stream -> encode on the handle's stream -> 8-byte size read-back
   for (size_t f = 0; f < n_frames; ++f) {
     if (!device_points) {
-      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(staged[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
+      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(slots[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
       CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f], e->pipe.h2d));
       CUDA_TRY(cudaStreamWaitEvent(e->stream, e->pipe.ev[2 * f], 0));
+      din[f] = slots[f];
     }
+    if (device_stage2) continue;
     if (int rc = encode_batch_device(e, 1, &din[f], &cloud_bytes[f], &dout[f], &caps[f], write_header)) return rc;
     CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p + f, e->d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
     CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f + 1], e->stream));
   }
-  // as soon as a frame's size is known, its blob goes down on the d2h stream (exactly `size` bytes)
+  if (device_stage2) {
+    if (int rc = encode_batch_device_stage2(e, n_frames, din.data(), cloud_bytes, dout.data(), caps, write_header)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+    if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+  }
   for (size_t f = 0; f < n_frames; ++f) {
-    CUDA_TRY(cudaEventSynchronize(e->pipe.ev[2 * f + 1]));
+    if (!device_stage2) CUDA_TRY(cudaEventSynchronize(e->pipe.ev[2 * f + 1]));
     const size_t sz = static_cast<size_t>(e->h_sizes.p[f]);
     if (sz > caps[f]) {  // the kernels refused the stores that did not fit and raised the error word
       if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
@@ -926,6 +854,138 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   }
   CUDA_TRY(cudaStreamSynchronize(e->pipe.d2h));
   return check_device_error(e->stream, e->d_err.p, e->h_err.p);
+}
+
+// Frames that passed check_encode_frame, through `route`. Device routes leave the blobs to the handle's stream and read
+// the sizes back only into a given written_host; host routes return with their blobs complete.
+static int encode_frames(cldn_encoder* e, EncodeRoute route, int mem, size_t n_frames, const void* const* clouds,
+                         const size_t* cloud_bytes, void* const* outs, const size_t* out_capacities, int write_header,
+                         size_t* written_host) {
+  const bool device_points = mem == CLDN_MEM_DEVICE_POINTS;
+  const size_t hdr = write_header ? e->header.size() : 0;
+  switch (route) {
+    case kEncDevice:
+      if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
+      return read_written(e, n_frames, written_host);
+    case kEncDeviceStage2:
+      if (int rc = encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
+      return read_written(e, n_frames, written_host);
+    case kEncHostPlain:
+    case kEncHostStage2: {
+      const bool stage2 = route == kEncHostStage2;
+      std::vector<size_t> caps(n_frames);
+      for (size_t f = 0; f < n_frames; ++f) {
+        caps[f] = (stage2 ? stage2_blob_staging : plain_blob_staging)(e, hdr, cloud_bytes[f], out_capacities[f]);
+      }
+      return encode_host_blobs(e, stage2, n_frames, clouds, cloud_bytes, outs, caps.data(), write_header, written_host, device_points);
+    }
+    case kEncHostLibrary:
+      // stage 1 into host scratch, then every chunk through the system's liblz4 / libzstd behind the header; frame by
+      // frame, so that the device staging holds one frame (the host compressor bounds this route, not the GPU)
+      for (size_t f = 0; f < n_frames; ++f) {
+        const size_t cap1 = stage1_arena_bytes(e, cloud_bytes[f] / e->info.point_step);
+        e->s2_tmp.resize(cap1);
+        void* s1_out = e->s2_tmp.data();
+        size_t s1 = 0;
+        if (int rc = encode_host_blobs(e, false, 1, &clouds[f], &cloud_bytes[f], &s1_out, &cap1, 0, &s1, device_points)) return rc;
+        uint8_t* out = static_cast<uint8_t*>(outs[f]);
+        if (hdr) memcpy(out, e->header.data(), hdr);
+        size_t w = 0;
+        if (int rc = stage2_compress_payload(e->stage2, e->s2_tmp.data(), s1, out + hdr, out_capacities[f] - hdr, &w)) return rc;
+        if (written_host) written_host[f] = hdr + w;
+      }
+      return CLDN_OK;
+  }
+  set_error("unknown encode route");
+  return CLDN_ERR_INTERNAL;
+}
+
+static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                             void* const* outs, const size_t* out_capacities, int write_header, size_t* written_host,
+                             int mem) {
+  if (!e || (n_frames && (!clouds || !cloud_bytes || !outs || !out_capacities))) {
+    set_error("null argument");
+    return CLDN_ERR_INVALID_ARGUMENT;
+  }
+  if (n_frames == 0) return CLDN_OK;
+  EncodeRoute route;
+  if (int rc = choose_encode_route(e, mem, &route)) return rc;
+  const size_t hdr = write_header ? e->header.size() : 0;
+  for (size_t f = 0; f < n_frames; ++f) {
+    if (int rc = check_encode_frame(e, hdr, clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return rc;
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  return encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header, written_host);
+}
+
+// Complete blobs of frames with their own dims: each frame's header is made on the host, the payloads are encoded behind
+// it (write_header = 0), and the headers are put in front of them afterwards (device blobs: one launch that also turns
+// the payload sizes into blob sizes; host blobs: memcpy). The handle's header is not touched.
+static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+                             const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
+                             size_t* written_host, int mem) {
+  if (!e || (n_frames && (!clouds || !cloud_bytes || !outs || !out_capacities))) {
+    set_error("null argument");
+    return CLDN_ERR_INVALID_ARGUMENT;
+  }
+  if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n_frames == 0) return CLDN_OK;
+  EncodeRoute route;
+  if (int rc = choose_encode_route(e, mem, &route)) return rc;
+  std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
+  std::vector<uint64_t> at(n_frames + 1, 0);
+  std::vector<void*> payload(n_frames);
+  std::vector<size_t> payload_cap(n_frames);
+  auto frame_error = [](size_t f, int rc) {
+    const std::string msg = cldn_b200_last_error();
+    set_error("frame %zu: %s", f, msg.c_str());
+    return rc;
+  };
+  for (size_t f = 0; f < n_frames; ++f) {
+    cldn_info_t fi = e->blob_info;
+    const size_t n = fi.point_step ? cloud_bytes[f] / fi.point_step : 0;
+    fi.width = widths ? widths[f] : static_cast<uint32_t>(n);
+    fi.height = heights ? heights[f] : 1u;
+    const std::vector<uint8_t> h = make_header(fi);
+    if (int rc = check_encode_frame(e, h.size(), clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return frame_error(f, rc);
+    if (static_cast<uint64_t>(fi.width) * fi.height != n) {
+      set_error("width * height (%u x %u) differs from the %zu points of the cloud", fi.width, fi.height, n);
+      return frame_error(f, CLDN_ERR_INVALID_ARGUMENT);
+    }
+    headers.insert(headers.end(), h.begin(), h.end());
+    at[f + 1] = headers.size();
+    payload[f] = static_cast<uint8_t*>(outs[f]) + h.size();
+    payload_cap[f] = out_capacities[f] - h.size();
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  if (mem != CLDN_MEM_DEVICE) {
+    std::vector<size_t> w(n_frames, 0);
+    if (int rc = encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data())) return rc;
+    for (size_t f = 0; f < n_frames; ++f) {
+      memcpy(outs[f], headers.data() + at[f], at[f + 1] - at[f]);
+      if (written_host) written_host[f] = (at[f + 1] - at[f]) + w[f];
+    }
+    return CLDN_OK;
+  }
+  if (int rc = encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, nullptr)) return rc;
+  const size_t tab_bytes = (2 * n_frames + 1) * sizeof(uint64_t) + headers.size();
+  uint8_t* ht = nullptr;
+  int slot = 0;
+  if (int rc = e->h_blob_headers.acquire(tab_bytes, &ht, &slot)) return rc;
+  if (int rc = e->d_blob_headers.reserve(tab_bytes)) return rc;
+  uint64_t* tab = reinterpret_cast<uint64_t*>(ht);
+  for (size_t f = 0; f < n_frames; ++f) tab[f] = reinterpret_cast<uintptr_t>(outs[f]);
+  memcpy(tab + n_frames, at.data(), (n_frames + 1) * sizeof(uint64_t));
+  memcpy(tab + 2 * n_frames + 1, headers.data(), headers.size());
+  CUDA_TRY(cudaMemcpyAsync(e->d_blob_headers.p, ht, tab_bytes, cudaMemcpyHostToDevice, e->stream));
+  if (int rc = e->h_blob_headers.commit(slot, e->stream)) return rc;
+  if (launch_place_headers(reinterpret_cast<const uint64_t*>(e->d_blob_headers.p), static_cast<uint32_t>(n_frames), e->d_sizes.p,
+                           e->stream) < 0) {
+    set_error("header launch failed");
+    return CLDN_ERR_CUDA;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return read_written(e, n_frames, written_host);
 }
 
 extern "C" {
@@ -942,92 +1002,6 @@ int cldn_b200_encode(cldn_encoder_t* enc, const void* cloud, size_t cloud_bytes,
   void* outs[1] = {out};
   return cldn_b200_encode_batch(enc, 1, clouds, &cloud_bytes, outs, &out_capacity, write_header, written, mem);
 }
-
-}  // extern "C"
-
-// Complete blobs of frames with their own dims: each frame's header is made on the host, the payloads are encoded by the
-// batch paths behind it (write_header = 0), and the headers are put in front of them afterwards (device pointers: one
-// launch that also turns the payload sizes into blob sizes; host pointers: memcpy). The handle's header is not touched.
-static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
-                             const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
-                             size_t* written_host, int mem) {
-  if (!e || (n_frames && (!clouds || !cloud_bytes || !outs || !out_capacities))) {
-    set_error("null argument");
-    return CLDN_ERR_INVALID_ARGUMENT;
-  }
-  if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
-  if (n_frames == 0) return CLDN_OK;
-  if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
-  if (mem == CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem)) {
-    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
-    return CLDN_ERR_UNSUPPORTED;
-  }
-  if (mem != CLDN_MEM_DEVICE && e->stage2 != CLDN_COMP_NONE && !stage2_device_codec(e, mem) && !g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
-  cldn_info_t full = e->info;
-  full.compression_opt = static_cast<uint8_t>(e->stage2);
-  std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
-  std::vector<uint64_t> at(n_frames + 1, 0);
-  std::vector<void*> payload(n_frames);
-  std::vector<size_t> payload_cap(n_frames);
-  auto frame_error = [](size_t f, int rc) {
-    const std::string msg = cldn_b200_last_error();
-    set_error("frame %zu: %s", f, msg.c_str());
-    return rc;
-  };
-  for (size_t f = 0; f < n_frames; ++f) {
-    const size_t n = full.point_step ? cloud_bytes[f] / full.point_step : 0;
-    cldn_info_t fi = full;
-    fi.width = widths ? widths[f] : static_cast<uint32_t>(n);
-    fi.height = heights ? heights[f] : 1u;
-    const std::vector<uint8_t> h = make_header(fi);
-    size_t need;
-    if (int rc = check_encode_frame(full, h.size(), cloud_bytes[f], out_capacities[f], &need)) return frame_error(f, rc);
-    if (n > 0xFFFFFFFFull) { set_error("too many points in one frame"); return frame_error(f, CLDN_ERR_UNSUPPORTED); }
-    if (static_cast<uint64_t>(fi.width) * fi.height != n) {
-      set_error("width * height (%u x %u) differs from the %zu points of the cloud", fi.width, fi.height, n);
-      return frame_error(f, CLDN_ERR_INVALID_ARGUMENT);
-    }
-    if (!outs[f] || (n > 0 && !clouds[f])) { set_error("null frame pointer"); return frame_error(f, CLDN_ERR_INVALID_ARGUMENT); }
-    headers.insert(headers.end(), h.begin(), h.end());
-    at[f + 1] = headers.size();
-    payload[f] = static_cast<uint8_t*>(outs[f]) + h.size();
-    payload_cap[f] = out_capacities[f] - h.size();
-  }
-  CUDA_TRY(cudaSetDevice(e->device));
-  if (mem != CLDN_MEM_DEVICE) {  // the blobs are host memory (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS)
-    std::vector<size_t> w(n_frames, 0);
-    if (int rc = encode_batch_impl(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data(), mem)) return rc;
-    for (size_t f = 0; f < n_frames; ++f) {
-      memcpy(outs[f], headers.data() + at[f], at[f + 1] - at[f]);
-      if (written_host) written_host[f] = (at[f + 1] - at[f]) + w[f];
-    }
-    return CLDN_OK;
-  }
-  const int rc = stage2_device_codec(e, mem)
-                     ? encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0)
-                     : encode_batch_device(e, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0);
-  if (rc) return rc;
-  const size_t tab_bytes = (2 * n_frames + 1) * sizeof(uint64_t) + headers.size();
-  uint8_t* ht = nullptr;
-  int slot = 0;
-  if (int rc2 = e->h_blob_headers.acquire(tab_bytes, &ht, &slot)) return rc2;
-  if (int rc2 = e->d_blob_headers.reserve(tab_bytes)) return rc2;
-  uint64_t* tab = reinterpret_cast<uint64_t*>(ht);
-  for (size_t f = 0; f < n_frames; ++f) tab[f] = reinterpret_cast<uintptr_t>(outs[f]);
-  memcpy(tab + n_frames, at.data(), (n_frames + 1) * sizeof(uint64_t));
-  memcpy(tab + 2 * n_frames + 1, headers.data(), headers.size());
-  CUDA_TRY(cudaMemcpyAsync(e->d_blob_headers.p, ht, tab_bytes, cudaMemcpyHostToDevice, e->stream));
-  if (int rc2 = e->h_blob_headers.commit(slot, e->stream)) return rc2;
-  if (launch_place_headers(reinterpret_cast<const uint64_t*>(e->d_blob_headers.p), static_cast<uint32_t>(n_frames), e->d_sizes.p,
-                           e->stream) < 0) {
-    set_error("header launch failed");
-    return CLDN_ERR_CUDA;
-  }
-  CUDA_TRY(cudaGetLastError());
-  return read_written(e, n_frames, written_host);
-}
-
-extern "C" {
 
 int cldn_b200_encode_blobs(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                            const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
