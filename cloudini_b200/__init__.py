@@ -19,7 +19,7 @@ from typing import List, Optional, Sequence
 
 __all__ = [
     "FieldType", "EncodingOptions", "CompressionOption", "PointField", "EncodingInfo", "EncodingInfoToYAML",
-    "EncodingInfoFromYAML", "EncodeHeader", "DecodeHeader", "MaxCompressedSize", "PointcloudEncoder",
+    "EncodingInfoFromYAML", "EncodeHeader", "DecodeHeader", "MaxCompressedSize", "PointcloudEncoder", "MixedEncoder",
     "PointcloudDecoder", "SizeOf", "lib", "library_path", "kernel_launch_count", "kDecodeButSkipStore",
 ]
 
@@ -143,6 +143,19 @@ def lib():
     L.cldn_b200_encoder_sizes_device.restype = vp
     L.cldn_b200_encoder_sync.argtypes = [vp]
     L.cldn_b200_encoder_set_stage2_on_device.argtypes = [vp, C.c_int]
+    L.cldn_b200_mixed_encoder_create.argtypes = [C.c_int, vp, C.POINTER(vp)]
+    L.cldn_b200_mixed_encoder_destroy.argtypes = [vp]
+    L.cldn_b200_mixed_encoder_destroy.restype = None
+    L.cldn_b200_mixed_encoder_set_stage2_on_device.argtypes = [vp, C.c_int]
+    L.cldn_b200_encode_mixed_blobs.argtypes = [vp, sz, C.POINTER(_CInfo), C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(sz),
+                                               C.c_int, C.POINTER(C.c_int32), C.POINTER(sz)]
+    L.cldn_b200_mixed_encoder_frame_error.argtypes = [vp, sz]
+    L.cldn_b200_mixed_encoder_frame_error.restype = C.c_char_p
+    L.cldn_b200_mixed_encoder_sizes_device.argtypes = [vp]
+    L.cldn_b200_mixed_encoder_sizes_device.restype = vp
+    L.cldn_b200_mixed_encoder_cached_layouts.argtypes = [vp]
+    L.cldn_b200_mixed_encoder_cached_layouts.restype = sz
+    L.cldn_b200_mixed_encoder_sync.argtypes = [vp]
     L.cldn_b200_decoder_create.argtypes = [C.c_int, vp, C.POINTER(vp)]
     L.cldn_b200_decoder_destroy.argtypes = [vp]
     L.cldn_b200_decoder_destroy.restype = None
@@ -441,6 +454,96 @@ class PointcloudEncoder:
 
     def sync(self):
         _check(lib().cldn_b200_encoder_sync(self._h))
+
+
+class MixedEncoder:
+    """Encodes batches of clouds of any mix of layouts (one EncodingInfo per frame) into complete blobs, with a status per
+    frame: blob f equals PointcloudEncoder(infos[f]).encode(cloud_f) with the header stating infos[f]'s width and height
+    ((points, 1) when both are 0). See cldn_b200_encode_mixed_blobs."""
+
+    def __init__(self, device: int = -1, stream: int = 0):
+        self._h = C.c_void_p()
+        _check(lib().cldn_b200_mixed_encoder_create(device, C.c_void_p(stream or None), C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            lib().cldn_b200_mixed_encoder_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_stage2_on_device(self, on: bool):
+        """As PointcloudEncoder.set_stage2_on_device, for every layout this handle encodes."""
+        _check(lib().cldn_b200_mixed_encoder_set_stage2_on_device(self._h, 1 if on else 0))
+
+    @staticmethod
+    def _cap(info: EncodingInfo, nbytes: int) -> int:
+        """MaxCompressedSize of the frame with its header, or 1 byte where that is not defined (point_step 0, a cloud
+        that is not a whole number of points, a bad layout), which the library then reports as that frame's error."""
+        step = info.point_step
+        if not step or nbytes % step:
+            return 1
+        w, h = (info.width, info.height) if info.width or info.height else (nbytes // step, 1)
+        try:
+            return MaxCompressedSize(replace(info, width=int(w), height=int(h)), nbytes // step, True)
+        except RuntimeError:
+            return 1
+
+    def _run(self, infos, in_ptrs, in_bytes, out_ptrs, out_caps, mem, want_sizes=True):
+        n = len(infos)
+        if not (len(in_ptrs) == len(in_bytes) == len(out_ptrs) == len(out_caps) == n):
+            raise RuntimeError("one info, cloud and output per frame")
+        m = max(n, 1)
+        status = (C.c_int32 * m)()
+        written = (C.c_size_t * m)() if want_sizes else None
+        rc = lib().cldn_b200_encode_mixed_blobs(self._h, n, (_CInfo * m)(*[_to_c(i) for i in infos]), (C.c_void_p * m)(*in_ptrs),
+                                                (C.c_size_t * m)(*in_bytes), (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps),
+                                                mem, status, written)
+        if rc and not any(status[f] for f in range(n)):   # refused as a whole (no handle): no frame has a status
+            _check(rc)
+        return [int(status[f]) for f in range(n)], ([int(written[f]) for f in range(n)] if want_sizes else None)
+
+    def _host_blobs(self, infos, in_ptrs, in_bytes, mem):
+        import numpy as np
+        caps = [self._cap(i, int(b)) for i, b in zip(infos, in_bytes)]
+        outs = [np.empty(max(c, 1), dtype=np.uint8) for c in caps]
+        status, sizes = self._run(infos, in_ptrs, in_bytes, [o.ctypes.data for o in outs], caps, mem)
+        return [(st, outs[f][:sizes[f]].tobytes() if st == 0 else None) for f, st in enumerate(status)]
+
+    def encode_blobs(self, clouds: Sequence, infos: Sequence[EncodingInfo]) -> list:
+        """Host clouds, one EncodingInfo each. Returns one (status, blob | None) per frame: status 0 or the negative
+        cldn_status_t that PointcloudEncoder(infos[f]) + encode_blobs give that frame alone (message: frame_error(f))."""
+        ins = [_host_ptr(c) for c in clouds]
+        r = self._host_blobs(infos, [p[0] for p in ins], [p[1] for p in ins], MEM_HOST)
+        del ins
+        return r
+
+    def encode_blobs_from_device(self, ptrs: Sequence[int], nbytes: Sequence[int], infos: Sequence[EncodingInfo]) -> list:
+        """encode_blobs of device-resident clouds (device addresses): the same (status, blob | None) list, host blobs."""
+        return self._host_blobs(infos, list(ptrs), list(nbytes), MEM_DEVICE_POINTS)
+
+    def encode_blobs_device(self, ptrs: Sequence[int], nbytes: Sequence[int], infos: Sequence[EncodingInfo], out_ptrs: Sequence[int],
+                            out_caps: Sequence[int], want_sizes: bool = True):
+        """Device clouds into device outputs. Returns (statuses, blob sizes); the sizes are None when want_sizes is False:
+        the call then returns once its work is enqueued, and the sizes are at sizes_device_ptr() after sync()."""
+        return self._run(infos, list(ptrs), list(nbytes), list(out_ptrs), list(out_caps), MEM_DEVICE, want_sizes)
+
+    def frame_error(self, f: int) -> str:
+        """Message of frame f of the last call ("" when it was encoded)."""
+        return lib().cldn_b200_mixed_encoder_frame_error(self._h, f).decode("utf-8", "replace")
+
+    def sizes_device_ptr(self) -> int:
+        return int(lib().cldn_b200_mixed_encoder_sizes_device(self._h) or 0)
+
+    def cached_layouts(self) -> int:
+        return int(lib().cldn_b200_mixed_encoder_cached_layouts(self._h))
+
+    def sync(self):
+        _check(lib().cldn_b200_mixed_encoder_sync(self._h))
 
 
 class PointcloudDecoder:

@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <stdexcept>
@@ -274,23 +275,29 @@ const char* dev_error_text(uint32_t code) {
 }  // namespace
 
 // =====================================================================================================================
-struct cldn_encoder {
+// What the kernels read about one layout: an encoder has one, a mixed encoder (cldn_b200_encode_mixed_blobs) one per
+// layout it has met.
+struct EncLayout {
   cldn_info_t info;       // as given, except compression_opt = NONE (what the GPU path produces)
   cldn_info_t blob_info;  // the blob's layout: as given, compression_opt as declared
   int stage2 = 0;         // the caller's compression_opt
-  bool stage2_on_device = false;  // cldn_b200_encoder_set_stage2_on_device
-  bool pooled = false;            // a handle of the per-thread pool (encoder_mark_pooled): keeps the libraries' bytes
-  std::vector<uint8_t> s2_tmp;
   Plan plan;
   std::vector<uint8_t> header;
+  uint32_t tile_points = 0;
+  DevBuf<Plan> d_plan;
+  DevBuf<uint8_t> d_header;
+};
+
+// The stream and the scratch of a handle, shared by every layout it encodes.
+struct EncScratch {
+  bool stage2_on_device = false;  // cldn_b200_encoder_set_stage2_on_device
+  std::vector<uint8_t> s2_tmp;
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  uint32_t tile_points = 0;
   uint32_t epoch = 0;
+  size_t sizes_at = 0;  // first d_sizes slot of the frames being encoded (cldn_b200_encode_mixed_blobs: of the group)
 
-  DevBuf<Plan> d_plan;
-  DevBuf<uint8_t> d_header;
   DevBuf<uint64_t> d_status;
   DevBuf<uint32_t> d_ticket;  // tile ticket of the persistent XYZI kernel
   DevBuf<EncFrame> d_frames;
@@ -321,6 +328,41 @@ struct cldn_encoder {
   DevBuf<uint8_t> d_blob_headers;
   PinRing<uint8_t> h_blob_headers;
 };
+
+struct cldn_encoder : EncLayout, EncScratch {
+  bool pooled = false;  // a handle of the per-thread pool (encoder_mark_pooled): keeps the libraries' bytes
+};
+
+// cldn_b200_encoder_create's refusals, in its order, and the host part of the layout of `info`.
+static int plan_layout(const cldn_info_t& info, EncLayout& l) {
+  Plan plan;
+  if (int rc = build_encode_plan(info, &plan)) return rc;
+  if (!plan.supported) {
+    set_error("EncodingInfo contains a field encoder this build cannot run");
+    return CLDN_ERR_UNSUPPORTED;
+  }
+  if (info.compression_opt > CLDN_COMP_ZSTD) { set_error("Unsupported compression option"); return CLDN_ERR_INVALID_ARGUMENT; }
+  // ZSTD exists only as the host library; LZ4 also runs on the device, so a missing liblz4 only matters to the host-pointer API
+  if (info.compression_opt == CLDN_COMP_ZSTD && !g_stage2.load(info.compression_opt)) return CLDN_ERR_UNSUPPORTED;
+  l.info = info;
+  l.blob_info = info;
+  l.stage2 = info.compression_opt;        // the header declares it; the kernels always produce stage 1
+  l.info.compression_opt = CLDN_COMP_NONE;
+  l.plan = plan;
+  l.header = make_header(info);
+  l.tile_points = choose_tile_points(plan);
+  return CLDN_OK;
+}
+
+// The device copies of the plan and the header (synchronous).
+static int upload_layout(EncLayout& l) {
+  if (int rc = l.d_plan.reserve(1)) return rc;
+  if (int rc = l.d_header.reserve(l.header.size())) return rc;
+  cudaError_t ce = cudaMemcpy(l.d_plan.p, &l.plan, sizeof(Plan), cudaMemcpyHostToDevice);
+  if (ce == cudaSuccess) ce = cudaMemcpy(l.d_header.p, l.header.data(), l.header.size(), cudaMemcpyHostToDevice);
+  if (ce != cudaSuccess) { set_error("cudaMemcpy failed: %s", cudaGetErrorString(ce)); return CLDN_ERR_CUDA; }
+  return CLDN_OK;
+}
 
 // LZ4_COMPRESSBOUND (lz4.h): worst case of a block for n input bytes
 static size_t lz4_bound(size_t n) { return n + n / 255 + 16; }
@@ -381,25 +423,10 @@ int cldn_b200_bind_host_thread_to_device(int device) {
 int cldn_b200_encoder_create(const cldn_info_t* info, int device, void* stream, cldn_encoder_t** out) {
   if (!info || !out) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
   *out = nullptr;
-  Plan plan;
-  if (int rc = build_encode_plan(*info, &plan)) return rc;
-  if (!plan.supported) {
-    set_error("EncodingInfo contains a field encoder this build cannot run");
-    return CLDN_ERR_UNSUPPORTED;
-  }
-  if (info->compression_opt > CLDN_COMP_ZSTD) { set_error("Unsupported compression option"); return CLDN_ERR_INVALID_ARGUMENT; }
-  // ZSTD exists only as the host library; LZ4 also runs on the device, so a missing liblz4 only matters to the host-pointer API
-  if (info->compression_opt == CLDN_COMP_ZSTD && !g_stage2.load(info->compression_opt)) return CLDN_ERR_UNSUPPORTED;
-  if (int rc = select_device(device)) return rc;
   cldn_encoder* e = new cldn_encoder();
-  e->info = *info;
-  e->blob_info = *info;
-  e->stage2 = info->compression_opt;        // the header declares it; the kernels always produce stage 1
-  e->info.compression_opt = CLDN_COMP_NONE;
-  e->plan = plan;
-  e->header = make_header(*info);
+  if (int rc = plan_layout(*info, *e)) { delete e; return rc; }
+  if (int rc = select_device(device)) { delete e; return rc; }
   cudaGetDevice(&e->device);
-  e->tile_points = choose_tile_points(plan);
   if (stream) {
     e->stream = static_cast<cudaStream_t>(stream);
   } else {
@@ -410,15 +437,9 @@ int cldn_b200_encoder_create(const cldn_info_t* info, int device, void* stream, 
     }
     e->own_stream = true;
   }
-  int rc = e->d_plan.reserve(1);
-  if (!rc) rc = e->d_header.reserve(e->header.size());
+  int rc = upload_layout(*e);
   if (!rc) rc = e->d_err.reserve(1, true);
   if (!rc) rc = e->h_err.reserve(1);
-  if (!rc) {
-    cudaError_t ce = cudaMemcpy(e->d_plan.p, &e->plan, sizeof(Plan), cudaMemcpyHostToDevice);
-    if (ce == cudaSuccess) ce = cudaMemcpy(e->d_header.p, e->header.data(), e->header.size(), cudaMemcpyHostToDevice);
-    if (ce != cudaSuccess) { set_error("cudaMemcpy failed: %s", cudaGetErrorString(ce)); rc = CLDN_ERR_CUDA; }
-  }
   if (rc) { cldn_b200_encoder_destroy(e); return rc; }
   *out = e;
   return CLDN_OK;
@@ -499,9 +520,9 @@ static int guarded(Fn&& fn) {
 // The encoder's rules for one frame, which every entry point checks on all frames before it uploads or launches
 // anything: the reference's checks in its order (cloudini.cpp:523-534), then this library's own. `hdr` is the header
 // bytes written in front of the payload at `out`.
-static int check_encode_frame(const cldn_encoder* e, size_t hdr, const void* cloud, size_t cloud_bytes, const void* out,
+static int check_encode_frame(const EncLayout& l, size_t hdr, const void* cloud, size_t cloud_bytes, const void* out,
                               size_t out_capacity) {
-  const cldn_info_t& blob = e->blob_info;
+  const cldn_info_t& blob = l.blob_info;
   if (blob.point_step == 0) { set_error("point_step cannot be 0"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (cloud_bytes % blob.point_step != 0) { set_error("Input cloud_data size is not a multiple of point_step"); return CLDN_ERR_INVALID_ARGUMENT; }
   const size_t n = cloud_bytes / blob.point_step;
@@ -526,18 +547,18 @@ enum EncodeRoute {
 
 // The route for this encoder and memory kind, or the refusal. LZ4 runs on the device for device blobs; ZSTD, and LZ4
 // into host blobs, run on the device only when the caller asked for it (cldn_b200_encoder_set_stage2_on_device).
-static int choose_encode_route(const cldn_encoder* e, int mem, EncodeRoute* route) {
+static int choose_encode_route(const EncLayout& l, const EncScratch& s, int mem, EncodeRoute* route) {
   if (mem != CLDN_MEM_HOST && mem != CLDN_MEM_DEVICE && mem != CLDN_MEM_DEVICE_POINTS) { set_error("bad mem kind"); return CLDN_ERR_INVALID_ARGUMENT; }
   const bool device_blobs = mem == CLDN_MEM_DEVICE;
-  if (e->stage2 == CLDN_COMP_NONE) {
+  if (l.stage2 == CLDN_COMP_NONE) {
     *route = device_blobs ? kEncDevice : kEncHostPlain;
-  } else if (e->stage2_on_device || (device_blobs && e->stage2 == CLDN_COMP_LZ4)) {
+  } else if (s.stage2_on_device || (device_blobs && l.stage2 == CLDN_COMP_LZ4)) {
     *route = device_blobs ? kEncDeviceStage2 : kEncHostStage2;
   } else if (device_blobs) {
-    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", e->stage2);
+    set_error("compression_opt %d needs the host-pointer API: ZSTD is delegated to the host library (LZ4 runs on the device)", l.stage2);
     return CLDN_ERR_UNSUPPORTED;
   } else {
-    if (!g_stage2.load(e->stage2)) return CLDN_ERR_UNSUPPORTED;
+    if (!g_stage2.load(l.stage2)) return CLDN_ERR_UNSUPPORTED;
     *route = kEncHostLibrary;
   }
   return CLDN_OK;
@@ -545,39 +566,39 @@ static int choose_encode_route(const cldn_encoder* e, int mem, EncodeRoute* rout
 
 // The internal stage-1 arena of the compressed routes for a frame of n points: the stage-1 worst case plus 64 bytes per
 // chunk and 64 more.
-static size_t stage1_arena_bytes(const cldn_encoder* e, size_t n) {
+static size_t stage1_arena_bytes(const EncLayout& l, size_t n) {
   bool ok;
-  return max_compressed_size(e->info, n, false, &ok) + 64 * ((n + kChunkPoints - 1) / kChunkPoints + 1);
+  return max_compressed_size(l.info, n, false, &ok) + 64 * ((n + kChunkPoints - 1) / kChunkPoints + 1);
 }
 
 // Device staging of a plain host blob. A committed V5 mode can exceed the reference's own worst-case formula (DeltaRle on
 // a 64-bit field: 11 bytes per value against the 10 it budgets); the reference then succeeds iff the caller's buffer is
 // large enough. Stage with room for the real worst case, never more than the caller gave: the kernels check every store
 // against this bound.
-static size_t plain_blob_staging(const cldn_encoder* e, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
-  const size_t n = cloud_bytes / e->info.point_step;
+static size_t plain_blob_staging(const EncLayout& l, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
+  const size_t n = cloud_bytes / l.info.point_step;
   bool ok;
-  size_t worst = max_compressed_size(e->info, n, false, &ok) + hdr;
-  for (uint32_t s = 0; s < e->plan.n_sections; ++s) {
-    if (e->plan.sections[s].bpv == 8) worst += n + 16 * (n / kChunkPoints + 1);
+  size_t worst = max_compressed_size(l.info, n, false, &ok) + hdr;
+  for (uint32_t s = 0; s < l.plan.n_sections; ++s) {
+    if (l.plan.sections[s].bpv == 8) worst += n + 16 * (n / kChunkPoints + 1);
   }
   return std::min(out_capacity, worst);
 }
 
 // Device staging of a host blob whose stage 2 runs on the device: a blob never exceeds its stage-1 arena plus the codec's
 // framing. Never more than the caller gave.
-static size_t stage2_blob_staging(const cldn_encoder* e, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
-  const size_t n = cloud_bytes / e->info.point_step, s1 = stage1_arena_bytes(e, n);
+static size_t stage2_blob_staging(const EncLayout& l, size_t hdr, size_t cloud_bytes, size_t out_capacity) {
+  const size_t n = cloud_bytes / l.info.point_step, s1 = stage1_arena_bytes(l, n);
   return std::min(out_capacity, hdr + s1 + s1 / 128 + 32 * ((n + kChunkPoints - 1) / kChunkPoints) + 256);
 }
 
 // Device-pointer batches: the blob sizes into written_host, if asked for (one read-back, synchronises).
-static int read_written(cldn_encoder* e, size_t n_frames, size_t* written_host) {
+static int read_written(EncScratch& s, size_t n_frames, size_t* written_host) {
   if (!written_host) return CLDN_OK;
-  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
-  CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-  if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
-  for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(e->h_sizes.p[f]);
+  if (int rc = s.h_sizes.reserve(n_frames)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.h_sizes.p, s.d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
+  if (int rc = check_device_error(s.stream, s.d_err.p, s.h_err.p)) return rc;
+  for (size_t f = 0; f < n_frames; ++f) written_host[f] = static_cast<size_t>(s.h_sizes.p[f]);
   return CLDN_OK;
 }
 
@@ -598,16 +619,16 @@ static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std
 
 // Stage 1 of frames that passed check_encode_frame, or of staging their caller sized: fills their EncFrames and enqueues
 // the kernels. Inputs and outputs are device pointers; the kernels check every store against out_capacities.
-static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                                void* const* outs, const size_t* out_capacities, int write_header) {
-  const cldn_info_t& info = e->info;
+  const cldn_info_t& info = l.info;
   EncFrame* hf = nullptr;
   int hf_slot = 0;
-  if (int rc = e->h_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
-  if (int rc = e->d_frames.reserve(n_frames)) return rc;
-  if (int rc = e->d_sizes.reserve(n_frames)) return rc;
-  const uint32_t T = e->tile_points;
-  const size_t hdr = write_header ? e->header.size() : 0;
+  if (int rc = s.h_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
+  if (int rc = s.d_frames.reserve(n_frames)) return rc;
+  if (int rc = s.d_sizes.reserve(s.sizes_at + n_frames)) return rc;
+  const uint32_t T = l.tile_points;
+  const size_t hdr = write_header ? l.header.size() : 0;
   uint64_t tiles = 0, chunks = 0;
   bool aligned16 = true;
   for (size_t f = 0; f < n_frames; ++f) {
@@ -627,101 +648,101 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
   }
   if (tiles > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
   for (size_t f = 0; f < n_frames; ++f) hf[f].side = nullptr;
-  if (e->plan.n_gorilla > 0) {
+  if (l.plan.n_gorilla > 0) {
     // FieldEncoderFloat_Gorilla keeps a leading/trailing-zero window across the points of a chunk: a pre-pass walks
     // every chunk in order and leaves one 12-byte record per (op, point) for the (parallel) regular kernel to copy
     size_t total_points = 0;
     for (size_t f = 0; f < n_frames; ++f) total_points += hf[f].n_points;
-    if (int rc = e->d_gorilla.reserve(total_points * 12 * e->plan.n_gorilla + 16)) return rc;
+    if (int rc = s.d_gorilla.reserve(total_points * 12 * l.plan.n_gorilla + 16)) return rc;
     size_t at = 0;
     for (size_t f = 0; f < n_frames; ++f) {
-      hf[f].side = e->d_gorilla.p + at;
-      at += static_cast<size_t>(hf[f].n_points) * 12 * e->plan.n_gorilla;
+      hf[f].side = s.d_gorilla.p + at;
+      at += static_cast<size_t>(hf[f].n_points) * 12 * l.plan.n_gorilla;
     }
   }
-  if (int rc = e->d_status.reserve(static_cast<size_t>(tiles) + 1, true)) return rc;
-  if (int rc = e->d_ticket.reserve(1)) return rc;
-  e->epoch = (e->epoch + 1) & 0x3FFFFFu;
-  if (e->epoch == 0) {  // epoch wrapped: stale words could alias
-    CUDA_TRY(cudaMemsetAsync(e->d_status.p, 0, e->d_status.cap * sizeof(uint64_t), e->stream));
-    e->epoch = 1;
+  if (int rc = s.d_status.reserve(static_cast<size_t>(tiles) + 1, true)) return rc;
+  if (int rc = s.d_ticket.reserve(1)) return rc;
+  s.epoch = (s.epoch + 1) & 0x3FFFFFu;
+  if (s.epoch == 0) {  // epoch wrapped: stale words could alias
+    CUDA_TRY(cudaMemsetAsync(s.d_status.p, 0, s.d_status.cap * sizeof(uint64_t), s.stream));
+    s.epoch = 1;
   }
   EncLaunch L;
-  L.frames = e->d_frames.p;
+  L.frames = s.d_frames.p;
   L.n_frames = static_cast<uint32_t>(n_frames);
   L.n_tiles_total = static_cast<uint32_t>(tiles);
-  L.plan = e->d_plan.p;
-  L.header = e->d_header.p;
+  L.plan = l.d_plan.p;
+  L.header = l.d_header.p;
   L.header_bytes = static_cast<uint32_t>(hdr);
-  L.status = e->d_status.p;
-  L.epoch = e->epoch;
-  L.sizes = e->d_sizes.p;
-  L.err = e->d_err.p;
+  L.status = s.d_status.p;
+  L.epoch = s.epoch;
+  L.sizes = s.d_sizes.p + s.sizes_at;
+  L.err = s.d_err.p;
   L.tile_points = T;
   L.flags = aligned16 ? kEncInputsAligned16 : 0u;
   L.uniform_tiles = 0;
-  L.tile_ticket = e->d_ticket.p;
+  L.tile_ticket = s.d_ticket.p;
   if (n_frames > 0 && hf[0].n_tiles > 0) {
     bool uniform = true;
     for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_tiles == hf[0].n_tiles;
     if (uniform) L.uniform_tiles = hf[0].n_tiles;
   }
 
-  if (e->plan.n_sections > 0) {
+  if (l.plan.n_sections > 0) {
     // V5: adaptive integer sections are produced first (they determine where every later chunk starts).
-    const uint32_t ns = e->plan.n_sections;
+    const uint32_t ns = l.plan.n_sections;
     // worst case of any mode is DeltaRle with one run per value: 5 + n * (max varint of the field + 1) bytes
     uint32_t per_value = 0;
-    for (uint32_t s = 0; s < ns; ++s) {
-      const uint32_t bpv = e->plan.sections[s].bpv;
+    for (uint32_t k = 0; k < ns; ++k) {
+      const uint32_t bpv = l.plan.sections[k].bpv;
       per_value = std::max<uint32_t>(per_value, (bpv == 2 ? 3u : bpv == 4 ? 5u : 10u) + 1u);
     }
     const uint32_t stride = 32 + kChunkPoints * per_value;   // 5 header bytes + 16 bytes the vector copy of place_sections_kernel may read past the end
-    if (int rc = e->d_modes.reserve(n_frames * ns)) return rc;
-    if (int rc = e->d_sec_scratch.reserve(static_cast<size_t>(chunks) * ns * stride)) return rc;
-    if (int rc = e->d_sec_sizes.reserve(static_cast<size_t>(chunks) * ns + 1)) return rc;
-    if (int rc = e->d_sec_excl.reserve(static_cast<size_t>(chunks) + n_frames + 1)) return rc;
+    if (int rc = s.d_modes.reserve(n_frames * ns)) return rc;
+    if (int rc = s.d_sec_scratch.reserve(static_cast<size_t>(chunks) * ns * stride)) return rc;
+    if (int rc = s.d_sec_sizes.reserve(static_cast<size_t>(chunks) * ns + 1)) return rc;
+    if (int rc = s.d_sec_excl.reserve(static_cast<size_t>(chunks) + n_frames + 1)) return rc;
     uint32_t* hcf = nullptr;
     int hcf_slot = 0;
-    if (int rc = e->h_chunk_frame.acquire(static_cast<size_t>(chunks) + n_frames + 1, &hcf, &hcf_slot)) return rc;
-    if (int rc = e->d_chunk_frame.reserve(static_cast<size_t>(chunks) + n_frames + 1)) return rc;
-    if (int rc = e->d_hash.reserve(palette_overflow_scratch_bytes() / 8 + 16)) return rc;
+    if (int rc = s.h_chunk_frame.acquire(static_cast<size_t>(chunks) + n_frames + 1, &hcf, &hcf_slot)) return rc;
+    if (int rc = s.d_chunk_frame.reserve(static_cast<size_t>(chunks) + n_frames + 1)) return rc;
+    if (int rc = s.d_hash.reserve(palette_overflow_scratch_bytes() / 8 + 16)) return rc;
     uint32_t cb = 0;
     for (size_t f = 0; f < n_frames; ++f) {
       EncFrame& F = hf[f];
-      F.sec_excl = e->d_sec_excl.p + cb + f;  // (n_chunks + 1) entries per frame
+      F.sec_excl = s.d_sec_excl.p + cb + f;  // (n_chunks + 1) entries per frame
       for (uint32_t c = 0; c < F.n_chunks; ++c) hcf[cb + c] = static_cast<uint32_t>(f);
       hcf[chunks + f] = cb;  // chunk_first[f]
       cb += F.n_chunks;
     }
-    CUDA_TRY(cudaMemcpyAsync(e->d_chunk_frame.p, hcf, (chunks + n_frames) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = e->h_chunk_frame.commit(hcf_slot, e->stream)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(e->d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = e->h_frames.commit(hf_slot, e->stream)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(s.d_chunk_frame.p, hcf, (chunks + n_frames) * sizeof(uint32_t), cudaMemcpyHostToDevice, s.stream));
+    if (int rc = s.h_chunk_frame.commit(hcf_slot, s.stream)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(s.d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, s.stream));
+    if (int rc = s.h_frames.commit(hf_slot, s.stream)) return rc;
     SecLaunch S{};
-    S.frames = e->d_frames.p;
+    S.frames = s.d_frames.p;
     S.n_frames = static_cast<uint32_t>(n_frames);
     S.n_chunks_total = static_cast<uint32_t>(chunks);
-    S.chunk_frame = e->d_chunk_frame.p;
-    S.chunk_first = e->d_chunk_frame.p + chunks;
-    S.plan = e->d_plan.p;
-    S.modes = e->d_modes.p;
-    S.scratch = e->d_sec_scratch.p;
+    S.chunk_frame = s.d_chunk_frame.p;
+    S.chunk_first = s.d_chunk_frame.p + chunks;
+    S.plan = l.d_plan.p;
+    S.modes = s.d_modes.p;
+    S.scratch = s.d_sec_scratch.p;
     S.sec_stride = stride;
-    S.sec_sizes = e->d_sec_sizes.p;
-    S.sec_excl = e->d_sec_excl.p;
-    S.hash_scratch = e->d_hash.p;
-    S.err = e->d_err.p;
+    S.sec_sizes = s.d_sec_sizes.p;
+    S.sec_excl = s.d_sec_excl.p;
+    S.hash_scratch = s.d_hash.p;
+    S.err = s.d_err.p;
     S.header_bytes = static_cast<uint32_t>(hdr);
-    if (launch_encode_sections(e->plan, S, e->stream) < 0) { set_error("section kernel launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_gorilla_prepass(e->plan, L, e->stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_encode_regular(e->plan, L, e->stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_place_sections(e->plan, S, e->d_status.p, e->epoch, T, e->stream) < 0) { set_error("section placement launch failed"); return CLDN_ERR_CUDA; }
+    if (launch_encode_sections(l.plan, S, s.stream) < 0) { set_error("section kernel launch failed"); return CLDN_ERR_CUDA; }
+    if (launch_gorilla_prepass(l.plan, L, s.stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
+    if (launch_encode_regular(l.plan, L, s.stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
+    if (launch_place_sections(l.plan, S, s.d_status.p, s.epoch, T, s.stream) < 0) { set_error("section placement launch failed"); return CLDN_ERR_CUDA; }
   } else {
-    CUDA_TRY(cudaMemcpyAsync(e->d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = e->h_frames.commit(hf_slot, e->stream)) return rc;
-    if (launch_gorilla_prepass(e->plan, L, e->stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_encode_regular(e->plan, L, e->stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
+    CUDA_TRY(cudaMemcpyAsync(s.d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, s.stream));
+    if (int rc = s.h_frames.commit(hf_slot, s.stream)) return rc;
+    if (launch_gorilla_prepass(l.plan, L, s.stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
+    if (launch_encode_regular(l.plan, L, s.stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
   }
   CUDA_TRY(cudaGetLastError());
   return CLDN_OK;
@@ -730,17 +751,17 @@ static int encode_batch_device(cldn_encoder* e, size_t n_frames, const void* con
 // Stage 1 into an internal arena, then stage 2 on the device: one LZ4 block per chunk (cldn_lz4.cu) or one ZSTD frame
 // per chunk (cldn_zstd_enc.cu), the blobs packed behind their headers into outs (device memory). The codec chooses the
 // slots and the compress launch; the arena, the chunk tables and the pack are shared. Launches: stage 1 + 2.
-static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
+static int encode_batch_device_stage2(const EncLayout& l, EncScratch& s, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
                                       void* const* outs, const size_t* out_capacities, int write_header) {
-  const cldn_info_t& info = e->info;  // compression NONE: what the stage-1 kernels produce
-  const bool zstd = e->stage2 == CLDN_COMP_ZSTD;
-  const size_t hdr = write_header ? e->header.size() : 0;
+  const cldn_info_t& info = l.info;  // compression NONE: what the stage-1 kernels produce
+  const bool zstd = l.stage2 == CLDN_COMP_ZSTD;
+  const size_t hdr = write_header ? l.header.size() : 0;
   const size_t zblock = zstd_enc_block_bytes();
   std::vector<size_t> s1_cap(n_frames), blocks_per_chunk(n_frames);
   size_t chunks = 0, max_chunk = 0, pieces = 0;
   for (size_t f = 0; f < n_frames; ++f) {
     const size_t n = cloud_bytes[f] / info.point_step, nc = (n + kChunkPoints - 1) / kChunkPoints;
-    s1_cap[f] = stage1_arena_bytes(e, n);
+    s1_cap[f] = stage1_arena_bytes(l, n);
     chunks += nc;
     bool ok;
     const size_t chunk_bound = max_compressed_size(info, std::min<size_t>(n, kChunkPoints), false, &ok) + 64;
@@ -750,26 +771,26 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
   }
   if (chunks > 0x7FFFFFFFull || pieces > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
   std::vector<void*> s1_ptr;
-  if (int rc = stage_layout(e->d_s1, n_frames, s1_cap.data(), s1_ptr)) return rc;
-  if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, s1_ptr.data(), s1_cap.data(), 0)) return rc;
+  if (int rc = stage_layout(s.d_s1, n_frames, s1_cap.data(), s1_ptr)) return rc;
+  if (int rc = encode_batch_device(l, s, n_frames, clouds, cloud_bytes, s1_ptr.data(), s1_cap.data(), 0)) return rc;
   // chunk tables + slots: one per chunk (LZ4), one per block of a chunk's worst case (ZSTD)
   const size_t slot = zstd ? zstd_enc_slot_bytes() : (lz4_bound(max_chunk) + 15) & ~size_t(15);
   if (slot > 0xFFFFFFF0ull) { set_error("chunk too large for LZ4"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = e->d_lz_scratch.reserve(std::max<size_t>(pieces, 1) * slot)) return rc;
-  if (int rc = e->d_lz_chunk_sizes.reserve(pieces + 1)) return rc;
-  if (int rc = e->d_lz_chunk_frame.reserve(2 * chunks + 2)) return rc;  // chunk -> frame, then block_begin (ZSTD)
-  if (int rc = e->d_lz_frames.reserve(n_frames)) return rc;
+  if (int rc = s.d_lz_scratch.reserve(std::max<size_t>(pieces, 1) * slot)) return rc;
+  if (int rc = s.d_lz_chunk_sizes.reserve(pieces + 1)) return rc;
+  if (int rc = s.d_lz_chunk_frame.reserve(2 * chunks + 2)) return rc;  // chunk -> frame, then block_begin (ZSTD)
+  if (int rc = s.d_lz_frames.reserve(n_frames)) return rc;
   Lz4Frame* hf = nullptr; int hf_slot = 0;
   uint32_t* hcf = nullptr; int hcf_slot = 0;
-  if (int rc = e->h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
-  if (int rc = e->h_lz_chunk_frame.acquire(2 * chunks + 2, &hcf, &hcf_slot)) return rc;
+  if (int rc = s.h_lz_frames.acquire(n_frames, &hf, &hf_slot)) return rc;
+  if (int rc = s.h_lz_chunk_frame.acquire(2 * chunks + 2, &hcf, &hcf_slot)) return rc;
   uint32_t cb = 0, pb = 0;
   for (size_t f = 0; f < n_frames; ++f) {
     const size_t n = cloud_bytes[f] / info.point_step;
     Lz4Frame& F = hf[f];
     memset(&F, 0, sizeof(F));
     F.plain = static_cast<uint8_t*>(s1_ptr[f]);
-    F.plain_bytes = e->d_sizes.p + f;
+    F.plain_bytes = s.d_sizes.p + s.sizes_at + f;
     F.blob_out = static_cast<uint8_t*>(outs[f]);
     F.blob_cap = out_capacities[f];
     F.n_chunks = static_cast<uint32_t>((n + kChunkPoints - 1) / kChunkPoints);
@@ -782,25 +803,25 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
     cb += F.n_chunks;
   }
   hcf[2 * chunks] = pb;
-  CUDA_TRY(cudaMemcpyAsync(e->d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, e->stream));
-  if (int rc = e->h_lz_frames.commit(hf_slot, e->stream)) return rc;
-  CUDA_TRY(cudaMemcpyAsync(e->d_lz_chunk_frame.p, hcf, (2 * chunks + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
-  if (int rc = e->h_lz_chunk_frame.commit(hcf_slot, e->stream)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.d_lz_frames.p, hf, n_frames * sizeof(Lz4Frame), cudaMemcpyHostToDevice, s.stream));
+  if (int rc = s.h_lz_frames.commit(hf_slot, s.stream)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.d_lz_chunk_frame.p, hcf, (2 * chunks + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, s.stream));
+  if (int rc = s.h_lz_chunk_frame.commit(hcf_slot, s.stream)) return rc;
   Lz4Launch Z{};
-  Z.frames = e->d_lz_frames.p;
+  Z.frames = s.d_lz_frames.p;
   Z.n_frames = static_cast<uint32_t>(n_frames);
   Z.n_chunks_total = static_cast<uint32_t>(chunks);
-  Z.chunk_frame = e->d_lz_chunk_frame.p;
-  Z.scratch = e->d_lz_scratch.p;
+  Z.chunk_frame = s.d_lz_chunk_frame.p;
+  Z.scratch = s.d_lz_scratch.p;
   Z.slot_stride = static_cast<uint32_t>(slot);
-  Z.chunk_sizes = e->d_lz_chunk_sizes.p;
-  Z.sizes = e->d_sizes.p;   // the pack kernel overwrites the stage-1 sizes with the blob sizes (it runs after every reader)
-  Z.err = e->d_err.p;
+  Z.chunk_sizes = s.d_lz_chunk_sizes.p;
+  Z.sizes = s.d_sizes.p + s.sizes_at;   // the pack kernel overwrites the stage-1 sizes with the blob sizes (it runs after every reader)
+  Z.err = s.d_err.p;
   if (zstd) {
-    Z.block_begin = e->d_lz_chunk_frame.p + chunks;
+    Z.block_begin = s.d_lz_chunk_frame.p + chunks;
     Z.n_blocks_total = static_cast<uint32_t>(pieces);
-    if (launch_zstd_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
-  } else if (launch_lz4_compress(Z, e->d_header.p, static_cast<uint32_t>(hdr), e->stream) < 0) {
+    if (launch_zstd_compress(Z, l.d_header.p, static_cast<uint32_t>(hdr), s.stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  } else if (launch_lz4_compress(Z, l.d_header.p, static_cast<uint32_t>(hdr), s.stream) < 0) {
     set_error("LZ4 kernel launch failed");
     return CLDN_ERR_CUDA;
   }
@@ -813,85 +834,85 @@ static int encode_batch_device_stage2(cldn_encoder* e, size_t n_frames, const vo
 // exactly that many bytes come down on the d2h stream. Stage 1 alone is pipelined frame by frame: frame f is encoded
 // while later frames go up and earlier ones come down. Device stage 2 encodes the batch at once and is checked before
 // anything comes down.
-static int encode_host_blobs(cldn_encoder* e, bool device_stage2, size_t n_frames, const void* const* clouds,
+static int encode_host_blobs(const EncLayout& l, EncScratch& s, bool device_stage2, size_t n_frames, const void* const* clouds,
                              const size_t* cloud_bytes, void* const* outs, const size_t* caps, int write_header,
                              size_t* written_host, bool device_points) {
   std::vector<void*> slots, dout;
   std::vector<const void*> din(clouds, clouds + n_frames);
   if (!device_points) {
-    if (int rc = stage_layout(e->d_in, n_frames, cloud_bytes, slots)) return rc;
+    if (int rc = stage_layout(s.d_in, n_frames, cloud_bytes, slots)) return rc;
   }
-  if (int rc = stage_layout(e->d_out, n_frames, caps, dout)) return rc;
-  if (int rc = e->pipe.ensure(2 * n_frames)) return rc;
-  if (int rc = e->h_sizes.reserve(n_frames)) return rc;
+  if (int rc = stage_layout(s.d_out, n_frames, caps, dout)) return rc;
+  if (int rc = s.pipe.ensure(2 * n_frames)) return rc;
+  if (int rc = s.h_sizes.reserve(n_frames)) return rc;
   for (size_t f = 0; f < n_frames; ++f) {
     if (!device_points) {
-      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(slots[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, e->pipe.h2d));
-      CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f], e->pipe.h2d));
-      CUDA_TRY(cudaStreamWaitEvent(e->stream, e->pipe.ev[2 * f], 0));
+      if (cloud_bytes[f]) CUDA_TRY(cudaMemcpyAsync(slots[f], clouds[f], cloud_bytes[f], cudaMemcpyHostToDevice, s.pipe.h2d));
+      CUDA_TRY(cudaEventRecord(s.pipe.ev[2 * f], s.pipe.h2d));
+      CUDA_TRY(cudaStreamWaitEvent(s.stream, s.pipe.ev[2 * f], 0));
       din[f] = slots[f];
     }
     if (device_stage2) continue;
-    if (int rc = encode_batch_device(e, 1, &din[f], &cloud_bytes[f], &dout[f], &caps[f], write_header)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p + f, e->d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-    CUDA_TRY(cudaEventRecord(e->pipe.ev[2 * f + 1], e->stream));
+    if (int rc = encode_batch_device(l, s, 1, &din[f], &cloud_bytes[f], &dout[f], &caps[f], write_header)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(s.h_sizes.p + f, s.d_sizes.p, sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
+    CUDA_TRY(cudaEventRecord(s.pipe.ev[2 * f + 1], s.stream));
   }
   if (device_stage2) {
-    if (int rc = encode_batch_device_stage2(e, n_frames, din.data(), cloud_bytes, dout.data(), caps, write_header)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(e->h_sizes.p, e->d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-    if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+    if (int rc = encode_batch_device_stage2(l, s, n_frames, din.data(), cloud_bytes, dout.data(), caps, write_header)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(s.h_sizes.p, s.d_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream));
+    if (int rc = check_device_error(s.stream, s.d_err.p, s.h_err.p)) return rc;
   }
   for (size_t f = 0; f < n_frames; ++f) {
-    if (!device_stage2) CUDA_TRY(cudaEventSynchronize(e->pipe.ev[2 * f + 1]));
-    const size_t sz = static_cast<size_t>(e->h_sizes.p[f]);
+    if (!device_stage2) CUDA_TRY(cudaEventSynchronize(s.pipe.ev[2 * f + 1]));
+    const size_t sz = static_cast<size_t>(s.h_sizes.p[f]);
     if (sz > caps[f]) {  // the kernels refused the stores that did not fit and raised the error word
-      if (int rc = check_device_error(e->stream, e->d_err.p, e->h_err.p)) return rc;
+      if (int rc = check_device_error(s.stream, s.d_err.p, s.h_err.p)) return rc;
       set_error("Output buffer too small for uncompressed chunk");
       return CLDN_ERR_BUFFER_TOO_SMALL;
     }
-    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], sz, cudaMemcpyDeviceToHost, e->pipe.d2h));
+    if (sz) CUDA_TRY(cudaMemcpyAsync(outs[f], dout[f], sz, cudaMemcpyDeviceToHost, s.pipe.d2h));
     if (written_host) written_host[f] = sz;
   }
-  CUDA_TRY(cudaStreamSynchronize(e->pipe.d2h));
-  return check_device_error(e->stream, e->d_err.p, e->h_err.p);
+  CUDA_TRY(cudaStreamSynchronize(s.pipe.d2h));
+  return check_device_error(s.stream, s.d_err.p, s.h_err.p);
 }
 
 // Frames that passed check_encode_frame, through `route`. Device routes leave the blobs to the handle's stream and read
 // the sizes back only into a given written_host; host routes return with their blobs complete.
-static int encode_frames(cldn_encoder* e, EncodeRoute route, int mem, size_t n_frames, const void* const* clouds,
+static int encode_frames(const EncLayout& l, EncScratch& s, EncodeRoute route, int mem, size_t n_frames, const void* const* clouds,
                          const size_t* cloud_bytes, void* const* outs, const size_t* out_capacities, int write_header,
                          size_t* written_host) {
   const bool device_points = mem == CLDN_MEM_DEVICE_POINTS;
-  const size_t hdr = write_header ? e->header.size() : 0;
+  const size_t hdr = write_header ? l.header.size() : 0;
   switch (route) {
     case kEncDevice:
-      if (int rc = encode_batch_device(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
-      return read_written(e, n_frames, written_host);
+      if (int rc = encode_batch_device(l, s, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
+      return read_written(s, n_frames, written_host);
     case kEncDeviceStage2:
-      if (int rc = encode_batch_device_stage2(e, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
-      return read_written(e, n_frames, written_host);
+      if (int rc = encode_batch_device_stage2(l, s, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header)) return rc;
+      return read_written(s, n_frames, written_host);
     case kEncHostPlain:
     case kEncHostStage2: {
       const bool stage2 = route == kEncHostStage2;
       std::vector<size_t> caps(n_frames);
       for (size_t f = 0; f < n_frames; ++f) {
-        caps[f] = (stage2 ? stage2_blob_staging : plain_blob_staging)(e, hdr, cloud_bytes[f], out_capacities[f]);
+        caps[f] = (stage2 ? stage2_blob_staging : plain_blob_staging)(l, hdr, cloud_bytes[f], out_capacities[f]);
       }
-      return encode_host_blobs(e, stage2, n_frames, clouds, cloud_bytes, outs, caps.data(), write_header, written_host, device_points);
+      return encode_host_blobs(l, s, stage2, n_frames, clouds, cloud_bytes, outs, caps.data(), write_header, written_host, device_points);
     }
     case kEncHostLibrary:
       // stage 1 into host scratch, then every chunk through the system's liblz4 / libzstd behind the header; frame by
       // frame, so that the device staging holds one frame (the host compressor bounds this route, not the GPU)
       for (size_t f = 0; f < n_frames; ++f) {
-        const size_t cap1 = stage1_arena_bytes(e, cloud_bytes[f] / e->info.point_step);
-        e->s2_tmp.resize(cap1);
-        void* s1_out = e->s2_tmp.data();
+        const size_t cap1 = stage1_arena_bytes(l, cloud_bytes[f] / l.info.point_step);
+        s.s2_tmp.resize(cap1);
+        void* s1_out = s.s2_tmp.data();
         size_t s1 = 0;
-        if (int rc = encode_host_blobs(e, false, 1, &clouds[f], &cloud_bytes[f], &s1_out, &cap1, 0, &s1, device_points)) return rc;
+        if (int rc = encode_host_blobs(l, s, false, 1, &clouds[f], &cloud_bytes[f], &s1_out, &cap1, 0, &s1, device_points)) return rc;
         uint8_t* out = static_cast<uint8_t*>(outs[f]);
-        if (hdr) memcpy(out, e->header.data(), hdr);
+        if (hdr) memcpy(out, l.header.data(), hdr);
         size_t w = 0;
-        if (int rc = stage2_compress_payload(e->stage2, e->s2_tmp.data(), s1, out + hdr, out_capacities[f] - hdr, &w)) return rc;
+        if (int rc = stage2_compress_payload(l.stage2, s.s2_tmp.data(), s1, out + hdr, out_capacities[f] - hdr, &w)) return rc;
         if (written_host) written_host[f] = hdr + w;
       }
       return CLDN_OK;
@@ -909,13 +930,13 @@ static int encode_batch_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   }
   if (n_frames == 0) return CLDN_OK;
   EncodeRoute route;
-  if (int rc = choose_encode_route(e, mem, &route)) return rc;
+  if (int rc = choose_encode_route(*e, *e, mem, &route)) return rc;
   const size_t hdr = write_header ? e->header.size() : 0;
   for (size_t f = 0; f < n_frames; ++f) {
-    if (int rc = check_encode_frame(e, hdr, clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return rc;
+    if (int rc = check_encode_frame(*e, hdr, clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return rc;
   }
   CUDA_TRY(cudaSetDevice(e->device));
-  return encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header, written_host);
+  return encode_frames(*e, *e, route, mem, n_frames, clouds, cloud_bytes, outs, out_capacities, write_header, written_host);
 }
 
 // Complete blobs of frames with their own dims: each frame's header is made on the host, the payloads are encoded behind
@@ -931,7 +952,7 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   if (!widths != !heights) { set_error("widths and heights must both be given or both be NULL"); return CLDN_ERR_INVALID_ARGUMENT; }
   if (n_frames == 0) return CLDN_OK;
   EncodeRoute route;
-  if (int rc = choose_encode_route(e, mem, &route)) return rc;
+  if (int rc = choose_encode_route(*e, *e, mem, &route)) return rc;
   std::vector<uint8_t> headers;          // frame f's header: headers[at[f], at[f + 1])
   std::vector<uint64_t> at(n_frames + 1, 0);
   std::vector<void*> payload(n_frames);
@@ -947,7 +968,7 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     fi.width = widths ? widths[f] : static_cast<uint32_t>(n);
     fi.height = heights ? heights[f] : 1u;
     const std::vector<uint8_t> h = make_header(fi);
-    if (int rc = check_encode_frame(e, h.size(), clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return frame_error(f, rc);
+    if (int rc = check_encode_frame(*e, h.size(), clouds[f], cloud_bytes[f], outs[f], out_capacities[f])) return frame_error(f, rc);
     if (static_cast<uint64_t>(fi.width) * fi.height != n) {
       set_error("width * height (%u x %u) differs from the %zu points of the cloud", fi.width, fi.height, n);
       return frame_error(f, CLDN_ERR_INVALID_ARGUMENT);
@@ -960,14 +981,14 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   CUDA_TRY(cudaSetDevice(e->device));
   if (mem != CLDN_MEM_DEVICE) {
     std::vector<size_t> w(n_frames, 0);
-    if (int rc = encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data())) return rc;
+    if (int rc = encode_frames(*e, *e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, w.data())) return rc;
     for (size_t f = 0; f < n_frames; ++f) {
       memcpy(outs[f], headers.data() + at[f], at[f + 1] - at[f]);
       if (written_host) written_host[f] = (at[f + 1] - at[f]) + w[f];
     }
     return CLDN_OK;
   }
-  if (int rc = encode_frames(e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, nullptr)) return rc;
+  if (int rc = encode_frames(*e, *e, route, mem, n_frames, clouds, cloud_bytes, payload.data(), payload_cap.data(), 0, nullptr)) return rc;
   const size_t tab_bytes = (2 * n_frames + 1) * sizeof(uint64_t) + headers.size();
   uint8_t* ht = nullptr;
   int slot = 0;
@@ -985,7 +1006,7 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
     return CLDN_ERR_CUDA;
   }
   CUDA_TRY(cudaGetLastError());
-  return read_written(e, n_frames, written_host);
+  return read_written(*e, n_frames, written_host);
 }
 
 extern "C" {
@@ -1062,15 +1083,19 @@ struct cldn_decoder {
   std::vector<cldn_info_t> frame_infos;
 };
 
-static bool same_info(const cldn_info_t& a, const cldn_info_t& b) {
-  if (a.width != b.width || a.height != b.height || a.point_step != b.point_step || a.encoding_opt != b.encoding_opt ||
-      a.compression_opt != b.compression_opt || a.version != b.version || a.n_fields != b.n_fields) return false;
+static bool same_fields(const cldn_info_t& a, const cldn_info_t& b) {
+  if (a.point_step != b.point_step || a.encoding_opt != b.encoding_opt || a.compression_opt != b.compression_opt ||
+      a.version != b.version || a.n_fields != b.n_fields) return false;
   for (uint32_t i = 0; i < a.n_fields; ++i) {
     const cldn_field_t &x = a.fields[i], &y = b.fields[i];
     if (x.offset != y.offset || x.type != y.type || x.has_resolution != y.has_resolution ||
         (x.has_resolution && memcmp(&x.resolution, &y.resolution, 4) != 0)) return false;
   }
   return true;
+}
+
+static bool same_info(const cldn_info_t& a, const cldn_info_t& b) {
+  return a.width == b.width && a.height == b.height && same_fields(a, b);
 }
 
 // PointcloudDecoder::updateDecoders (cloudini.cpp:627-633)
@@ -1700,16 +1725,20 @@ static int read_blob_headers(cldn_decoder* d, size_t n, const void* const* blobs
   return CLDN_OK;
 }
 
+// The same layout, width and height aside: everything a plan and a header (but for its dims) depend on.
+static bool same_layout(const cldn_info_t& a, const cldn_info_t& b) {
+  if (!same_fields(a, b) || strncmp(a.encoding_config, b.encoding_config, sizeof(a.encoding_config)) != 0) return false;
+  for (uint32_t i = 0; i < a.n_fields; ++i) {
+    if (strncmp(a.fields[i].name, b.fields[i].name, CLDN_MAX_NAME) != 0) return false;
+  }
+  return true;
+}
+
 // Frames decoded by one fused launch: the same layout (width and height aside) and compression. LZ4 and ZSTD frames also
 // share the bound of a decompressed chunk, which depends on the points of a chunk, so that every frame is bounded
 // exactly as cldn_b200_decode bounds it.
 static bool same_group(const cldn_info_t& a, uint64_t a_points, const cldn_info_t& b, uint64_t b_points) {
-  cldn_info_t x = a, y = b;
-  x.width = y.width = x.height = y.height = 0;
-  if (!same_info(x, y) || strncmp(a.encoding_config, b.encoding_config, sizeof(a.encoding_config)) != 0) return false;
-  for (uint32_t i = 0; i < a.n_fields; ++i) {
-    if (strncmp(a.fields[i].name, b.fields[i].name, CLDN_MAX_NAME) != 0) return false;
-  }
+  if (!same_layout(a, b)) return false;
   return a.compression_opt == CLDN_COMP_NONE || std::min<uint64_t>(a_points, kChunkPoints) == std::min<uint64_t>(b_points, kChunkPoints);
 }
 
@@ -1901,6 +1930,307 @@ uint32_t cldn_b200_DecodeCompressedData(const void* encoded_data, uint32_t encod
                                   output_data, output_capacity, CLDN_MEM_HOST);
   cldn_b200_decoder_destroy(dec);
   return rc == CLDN_OK ? static_cast<uint32_t>(decoded) : 0;
+}
+
+}  // extern "C"
+
+// =====================================================================================================================
+// cldn_b200_encode_mixed_blobs: frames of any layouts through one handle, whose stream and scratch every layout shares.
+// The layouts of the last kMixedLayouts calls' frames are kept (plan, header, device plan), at least those of the call
+// in progress.
+constexpr size_t kMixedLayouts = 16;
+
+struct cldn_mixed_encoder : EncScratch {
+  struct Cached {
+    std::unique_ptr<EncLayout> layout;
+    uint64_t used = 0;  // the last call with a frame of this layout
+  };
+  std::vector<Cached> layouts;
+  uint64_t calls = 0;
+  DevBuf<uint64_t> d_blob_sizes;  // blob sizes of the last CLDN_MEM_DEVICE call, one per frame (0: not encoded)
+  std::vector<std::string> frame_errors;
+};
+
+// The layout of `info`, planned (cldn_b200_encoder_create's refusals) and uploaded the first time it is met.
+static int mixed_layout(cldn_mixed_encoder* m, const cldn_info_t& info, EncLayout** out) {
+  for (auto& c : m->layouts) {
+    if (same_layout(c.layout->blob_info, info)) {
+      c.used = m->calls;
+      *out = c.layout.get();
+      return CLDN_OK;
+    }
+  }
+  std::unique_ptr<EncLayout> l(new EncLayout());
+  if (int rc = plan_layout(info, *l)) return rc;
+  l->info.width = l->info.height = l->blob_info.width = l->blob_info.height = 0;  // every frame's header states its own
+  l->header = make_header(l->blob_info);
+  if (int rc = upload_layout(*l)) return rc;
+  *out = l.get();
+  m->layouts.push_back({std::move(l), m->calls});
+  return CLDN_OK;
+}
+
+// Drops the least recently used layouts beyond kMixedLayouts; an earlier asynchronous call may still read their plans.
+static int trim_layouts(cldn_mixed_encoder* m) {
+  if (m->layouts.size() <= kMixedLayouts) return CLDN_OK;
+  CUDA_TRY(cudaStreamSynchronize(m->stream));
+  std::sort(m->layouts.begin(), m->layouts.end(), [](const auto& a, const auto& b) { return a.used > b.used; });
+  m->layouts.resize(kMixedLayouts);
+  return CLDN_OK;
+}
+
+// Every frame gets the status cldn_b200_encoder_create(&infos[f]) + cldn_b200_encode_blobs give it alone: each is checked
+// on the host with its own layout, and the good frames go through the fused batch path of their layout and route, one
+// group after the other. Device blobs: the groups are enqueued back to back, one launch places every header and writes
+// every blob size, and the sizes are read back once (not at all without `written`). Host blobs: each group returns
+// complete, headers copied on the host. A group that fails on the device (which the worst-case capacities rule out) is
+// encoded again frame by frame, so that only the guilty frame gets the status.
+static int encode_mixed_impl(cldn_mixed_encoder* m, size_t n, const cldn_info_t* infos, const void* const* clouds,
+                             const size_t* cloud_bytes, void* const* outs, const size_t* caps, int mem, int32_t* status,
+                             size_t* written) {
+  if (!m || (n && !status)) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  m->frame_errors.assign(n, "frame not encoded");
+  for (size_t f = 0; f < n; ++f) {
+    status[f] = CLDN_ERR_INTERNAL;
+    if (written) written[f] = 0;
+  }
+  auto result = [&]() -> int {
+    for (size_t f = 0; f < n; ++f) {
+      if (status[f] != CLDN_OK) { set_error("frame %zu: %s", f, m->frame_errors[f].c_str()); return status[f]; }
+    }
+    return CLDN_OK;
+  };
+  auto fail = [&](size_t f, int rc) {
+    status[f] = rc;
+    m->frame_errors[f] = cldn_b200_last_error();
+  };
+  auto fail_all = [&](int rc) {
+    for (size_t f = 0; f < n; ++f) fail(f, rc);
+    return result();
+  };
+  if (n == 0) return CLDN_OK;
+  if (!infos || !clouds || !cloud_bytes || !outs || !caps) { set_error("null argument"); return fail_all(CLDN_ERR_INVALID_ARGUMENT); }
+  if (cudaSetDevice(m->device) != cudaSuccess) { set_error("cudaSetDevice failed"); return fail_all(CLDN_ERR_CUDA); }
+  ++m->calls;
+  if (int rc = trim_layouts(m)) return fail_all(rc);
+
+  std::vector<EncLayout*> layout(n, nullptr);
+  std::vector<EncodeRoute> route(n);
+  std::vector<uint8_t> headers;  // frame f's header: headers[at[f], at[f + 1])
+  std::vector<uint64_t> at(n + 1, 0);
+  std::vector<void*> payload(n);
+  std::vector<size_t> payload_cap(n);
+  std::vector<std::vector<size_t>> groups;  // good frames of one layout and route, in call order
+  for (size_t f = 0; f < n; ++f) {
+    at[f + 1] = at[f];
+    int rc = mixed_layout(m, infos[f], &layout[f]);
+    if (!rc) rc = choose_encode_route(*layout[f], *m, mem, &route[f]);
+    if (rc) { fail(f, rc); continue; }
+    cldn_info_t fi = layout[f]->blob_info;
+    const size_t pts = fi.point_step ? cloud_bytes[f] / fi.point_step : 0;
+    fi.width = infos[f].width;
+    fi.height = infos[f].height;
+    if (fi.width == 0 && fi.height == 0) { fi.width = static_cast<uint32_t>(pts); fi.height = 1; }
+    const std::vector<uint8_t> h = make_header(fi);
+    rc = check_encode_frame(*layout[f], h.size(), clouds[f], cloud_bytes[f], outs[f], caps[f]);
+    if (!rc && static_cast<uint64_t>(fi.width) * fi.height != pts) {
+      set_error("width * height (%u x %u) differs from the %zu points of the cloud", fi.width, fi.height, pts);
+      rc = CLDN_ERR_INVALID_ARGUMENT;
+    }
+    if (rc) { fail(f, rc); continue; }
+    headers.insert(headers.end(), h.begin(), h.end());
+    at[f + 1] = headers.size();
+    payload[f] = static_cast<uint8_t*>(outs[f]) + h.size();
+    payload_cap[f] = caps[f] - h.size();
+    auto g = std::find_if(groups.begin(), groups.end(), [&](const std::vector<size_t>& G) {
+      return layout[G[0]] == layout[f] && route[G[0]] == route[f];
+    });
+    if (g == groups.end()) groups.push_back({f});
+    else g->push_back(f);
+  }
+  // the arrays of one group's frames
+  std::vector<const void*> g_clouds;
+  std::vector<size_t> g_bytes, g_caps, g_written;
+  std::vector<void*> g_payload;
+  auto gather = [&](const std::vector<size_t>& G) {
+    g_clouds.clear(); g_bytes.clear(); g_caps.clear(); g_payload.clear();
+    for (size_t f : G) {
+      g_clouds.push_back(clouds[f]);
+      g_bytes.push_back(cloud_bytes[f]);
+      g_payload.push_back(payload[f]);
+      g_caps.push_back(payload_cap[f]);
+    }
+    g_written.assign(G.size(), 0);
+  };
+
+  if (mem != CLDN_MEM_DEVICE) {
+    auto run = [&](const std::vector<size_t>& G) -> int {
+      gather(G);
+      const size_t f0 = G[0];
+      if (int rc = encode_frames(*layout[f0], *m, route[f0], mem, G.size(), g_clouds.data(), g_bytes.data(), g_payload.data(),
+                                 g_caps.data(), 0, g_written.data())) return rc;
+      for (size_t i = 0; i < G.size(); ++i) {
+        const size_t f = G[i];
+        memcpy(outs[f], headers.data() + at[f], at[f + 1] - at[f]);
+        if (written) written[f] = (at[f + 1] - at[f]) + g_written[i];
+        status[f] = CLDN_OK;
+        m->frame_errors[f].clear();
+      }
+      return CLDN_OK;
+    };
+    for (const auto& G : groups) {
+      if (run(G) == CLDN_OK) continue;
+      for (size_t f : G) {
+        if (int rc = run(std::vector<size_t>(1, f))) fail(f, rc);
+      }
+    }
+    return result();
+  }
+
+  // device blobs: d_sizes holds the payload sizes group after group, d_blob_sizes the blob sizes frame by frame
+  size_t good = 0;
+  for (const auto& G : groups) good += G.size();
+  if (int rc = m->d_sizes.reserve(good)) return fail_all(rc);
+  if (int rc = m->d_blob_sizes.reserve(n)) return fail_all(rc);
+  if (int rc = m->h_sizes.reserve(n)) return fail_all(rc);
+  if (cudaMemsetAsync(m->d_blob_sizes.p, 0, n * sizeof(uint64_t), m->stream) != cudaSuccess) {
+    set_error("cudaMemsetAsync failed");
+    return fail_all(CLDN_ERR_CUDA);
+  }
+  auto enqueue = [&](const std::vector<std::vector<size_t>>& gs) -> int {
+    std::vector<size_t> placed;
+    std::vector<uint32_t> slots;
+    for (const auto& G : gs) {
+      gather(G);
+      const size_t f0 = G[0];
+      m->sizes_at = slots.size();
+      const int rc = encode_frames(*layout[f0], *m, route[f0], mem, G.size(), g_clouds.data(), g_bytes.data(), g_payload.data(),
+                                   g_caps.data(), 0, nullptr);
+      m->sizes_at = 0;
+      if (rc) return rc;
+      for (size_t f : G) {
+        placed.push_back(f);
+        slots.push_back(static_cast<uint32_t>(slots.size()));
+      }
+    }
+    const size_t np = placed.size();
+    for (size_t f : placed) slots.push_back(static_cast<uint32_t>(f));
+    // [np blob addresses][np + 1 header offsets][packed headers][pad][2 np slots]
+    size_t hbytes = 0;
+    for (size_t f : placed) hbytes += at[f + 1] - at[f];
+    const size_t slots_at = ((2 * np + 1) * sizeof(uint64_t) + hbytes + 7) & ~size_t(7);
+    const size_t tab_bytes = slots_at + slots.size() * sizeof(uint32_t);
+    uint8_t* ht = nullptr;
+    int slot = 0;
+    if (int rc = m->h_blob_headers.acquire(tab_bytes, &ht, &slot)) return rc;
+    if (int rc = m->d_blob_headers.reserve(tab_bytes)) return rc;
+    uint64_t* tab = reinterpret_cast<uint64_t*>(ht);
+    uint8_t* packed = ht + (2 * np + 1) * sizeof(uint64_t);
+    tab[np] = 0;
+    for (size_t i = 0; i < np; ++i) {
+      const size_t f = placed[i], hb = at[f + 1] - at[f];
+      tab[i] = reinterpret_cast<uintptr_t>(outs[f]);
+      memcpy(packed + tab[np + i], headers.data() + at[f], hb);
+      tab[np + i + 1] = tab[np + i] + hb;
+    }
+    memcpy(ht + slots_at, slots.data(), slots.size() * sizeof(uint32_t));
+    CUDA_TRY(cudaMemcpyAsync(m->d_blob_headers.p, ht, tab_bytes, cudaMemcpyHostToDevice, m->stream));
+    if (int rc = m->h_blob_headers.commit(slot, m->stream)) return rc;
+    if (launch_place_headers(reinterpret_cast<const uint64_t*>(m->d_blob_headers.p), static_cast<uint32_t>(np), m->d_blob_sizes.p,
+                             m->stream, m->d_sizes.p, reinterpret_cast<const uint32_t*>(m->d_blob_headers.p + slots_at)) < 0) {
+      set_error("header launch failed");
+      return CLDN_ERR_CUDA;
+    }
+    CUDA_TRY(cudaGetLastError());
+    return CLDN_OK;
+  };
+  auto read_back = [&]() -> int {
+    CUDA_TRY(cudaMemcpyAsync(m->h_sizes.p, m->d_blob_sizes.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, m->stream));
+    return check_device_error(m->stream, m->d_err.p, m->h_err.p);
+  };
+  auto done = [&](size_t f) {
+    status[f] = CLDN_OK;
+    m->frame_errors[f].clear();
+    if (written) written[f] = static_cast<size_t>(m->h_sizes.p[f]);
+  };
+  int rc = enqueue(groups);
+  if (rc == CLDN_OK && written) rc = read_back();
+  if (rc == CLDN_OK) {
+    for (const auto& G : groups) {
+      for (size_t f : G) done(f);
+    }
+    return result();
+  }
+  for (const auto& G : groups) {
+    for (size_t f : G) {
+      int rf = enqueue(std::vector<std::vector<size_t>>(1, std::vector<size_t>(1, f)));
+      if (!rf) rf = read_back();
+      if (rf) fail(f, rf);
+      else done(f);
+    }
+  }
+  return result();
+}
+
+extern "C" {
+
+int cldn_b200_mixed_encoder_create(int device, void* stream, cldn_mixed_encoder_t** out) {
+  if (!out) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  *out = nullptr;
+  if (int rc = select_device(device)) return rc;
+  cldn_mixed_encoder* m = new cldn_mixed_encoder();
+  cudaGetDevice(&m->device);
+  if (stream) {
+    m->stream = static_cast<cudaStream_t>(stream);
+  } else {
+    if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) {
+      set_error("cudaStreamCreate failed");
+      delete m;
+      return CLDN_ERR_CUDA;
+    }
+    m->own_stream = true;
+  }
+  int rc = m->d_err.reserve(1, true);
+  if (!rc) rc = m->h_err.reserve(1);
+  if (rc) { cldn_b200_mixed_encoder_destroy(m); return rc; }
+  *out = m;
+  return CLDN_OK;
+}
+
+void cldn_b200_mixed_encoder_destroy(cldn_mixed_encoder_t* m) {
+  if (!m) return;
+  cudaSetDevice(m->device);
+  if (m->stream) cudaStreamSynchronize(m->stream);
+  const cudaStream_t own = m->own_stream ? m->stream : nullptr;
+  delete m;  // the buffers and the layouts free themselves
+  if (own) cudaStreamDestroy(own);
+}
+
+int cldn_b200_mixed_encoder_set_stage2_on_device(cldn_mixed_encoder_t* m, int on) {
+  if (!m) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (on != 0 && on != 1) { set_error("on must be 0 or 1"); return CLDN_ERR_INVALID_ARGUMENT; }
+  m->stage2_on_device = on == 1;
+  return CLDN_OK;
+}
+
+int cldn_b200_encode_mixed_blobs(cldn_mixed_encoder_t* m, size_t n_frames, const cldn_info_t* infos, const void* const* clouds,
+                                 const size_t* cloud_bytes, void* const* outs, const size_t* out_capacities, int mem,
+                                 int32_t* status, size_t* written) {
+  return guarded([&] { return encode_mixed_impl(m, n_frames, infos, clouds, cloud_bytes, outs, out_capacities, mem, status, written); });
+}
+
+const char* cldn_b200_mixed_encoder_frame_error(const cldn_mixed_encoder_t* m, size_t f) {
+  return m && f < m->frame_errors.size() ? m->frame_errors[f].c_str() : "";
+}
+
+const uint64_t* cldn_b200_mixed_encoder_sizes_device(const cldn_mixed_encoder_t* m) { return m ? m->d_blob_sizes.p : nullptr; }
+
+size_t cldn_b200_mixed_encoder_cached_layouts(const cldn_mixed_encoder_t* m) { return m ? m->layouts.size() : 0; }
+
+int cldn_b200_mixed_encoder_sync(cldn_mixed_encoder_t* m) {
+  if (!m) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  CUDA_TRY(cudaSetDevice(m->device));
+  return check_device_error(m->stream, m->d_err.p, m->h_err.p);
 }
 
 }  // extern "C"

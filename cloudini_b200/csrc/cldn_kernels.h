@@ -206,8 +206,10 @@ int launch_zstd_decompress(const ZstdLaunch& Z, cudaStream_t stream);
 // One launch: tab = [n source addresses][n byte counts][n offsets into dst]; blob f's bytes go to dst + offset[f].
 int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaStream_t stream);
 // Headers of blobs encoded without one (cldn_b200_encode_blobs), one launch: tab = [n blob addresses][n + 1 offsets into
-// the packed header bytes][packed header bytes]; header f is copied to blob f and its length added to sizes[f].
-int launch_place_headers(const uint64_t* tab, uint32_t n, uint64_t* sizes, cudaStream_t stream);
+// the packed header bytes][packed header bytes]; header f is copied to blob f and its length added to sizes[f]. With
+// `slots` (2n words, cldn_b200_encode_mixed_blobs): sizes[slots[n + f]] = from[slots[f]] + that length instead.
+int launch_place_headers(const uint64_t* tab, uint32_t n, uint64_t* sizes, cudaStream_t stream, const uint64_t* from = nullptr,
+                         const uint32_t* slots = nullptr);
 
 uint64_t kernel_launch_count();
 void count_launch(int n = 1);  // process-wide, atomic: handles on other threads count into the same total

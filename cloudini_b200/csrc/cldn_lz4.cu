@@ -331,18 +331,23 @@ int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaSt
 }
 
 // One CTA per blob; tab holds n destination addresses and n + 1 offsets into the packed header bytes that follow it.
-// Blob f's header goes in front of its payload, and the payload size in sizes[f] becomes the blob size.
-__global__ void __launch_bounds__(256) place_headers_kernel(const uint64_t* tab, uint32_t n, uint64_t* sizes) {
+// Blob f's header goes in front of its payload, and the payload size in sizes[f] becomes the blob size. With `slots`
+// (2n words), the payload size is from[slots[f]] and the blob size goes to sizes[slots[n + f]].
+__global__ void __launch_bounds__(256) place_headers_kernel(const uint64_t* tab, uint32_t n, uint64_t* sizes, const uint64_t* from,
+                                                            const uint32_t* slots) {
   const uint32_t f = blockIdx.x;
   const uint8_t* packed = reinterpret_cast<const uint8_t*>(tab + 2ull * n + 1);
   const uint64_t begin = tab[n + f], bytes = tab[n + f + 1] - begin;
   lz_copy(reinterpret_cast<uint8_t*>(tab[f]), packed + begin, static_cast<uint32_t>(bytes), threadIdx.x, blockDim.x);
-  if (threadIdx.x == 0) sizes[f] += bytes;
+  if (threadIdx.x != 0) return;
+  if (slots) sizes[slots[n + f]] = from[slots[f]] + bytes;
+  else sizes[f] += bytes;
 }
 
-int launch_place_headers(const uint64_t* tab, uint32_t n, uint64_t* sizes, cudaStream_t stream) {
+int launch_place_headers(const uint64_t* tab, uint32_t n, uint64_t* sizes, cudaStream_t stream, const uint64_t* from,
+                         const uint32_t* slots) {
   if (n == 0) return 0;
-  place_headers_kernel<<<n, 256, 0, stream>>>(tab, n, sizes);
+  place_headers_kernel<<<n, 256, 0, stream>>>(tab, n, sizes, from, slots);
   count_launch(1);
   return 1;
 }

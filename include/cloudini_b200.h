@@ -109,6 +109,7 @@ typedef struct cldn_info_t {
 
 typedef struct cldn_encoder cldn_encoder_t; /* replaces Cloudini::PointcloudEncoder (cloudini.hpp:154-211) */
 typedef struct cldn_decoder cldn_decoder_t; /* replaces Cloudini::PointcloudDecoder (cloudini.hpp:216-244) */
+typedef struct cldn_mixed_encoder cldn_mixed_encoder_t; /* encoder of frames of any layouts (cldn_b200_encode_mixed_blobs) */
 
 /* ---- library ------------------------------------------------------------------------------------------------- */
 const char* cldn_b200_version(void);
@@ -204,6 +205,46 @@ int cldn_b200_encoder_set_dims(cldn_encoder_t* enc, uint32_t width, uint32_t hei
 int cldn_b200_encoder_set_stage2_on_device(cldn_encoder_t* enc, int on);
 /* Waits for everything enqueued on the handle's stream; reports device-side errors of the last call. */
 int cldn_b200_encoder_sync(cldn_encoder_t* enc);
+
+/* ---- mixed-layout encoder ------------------------------------------------------------------------------------- */
+/* A handle that is not tied to one layout, as the decoder is not (no reference counterpart: the reference builds a
+ * PointcloudEncoder per message). One stream (`stream` as for cldn_b200_encoder_create), one set of device and pinned
+ * buffers for every layout, and the plans of the layouts met in the last calls (at least 16). Not thread-safe. */
+int cldn_b200_mixed_encoder_create(int device, void* stream, cldn_mixed_encoder_t** out);
+void cldn_b200_mixed_encoder_destroy(cldn_mixed_encoder_t* m);
+/* 0 (default) / 1: as cldn_b200_encoder_set_stage2_on_device, for every layout this handle encodes. */
+int cldn_b200_mixed_encoder_set_stage2_on_device(cldn_mixed_encoder_t* m, int on);
+/* Complete blobs of clouds in any mix of layouts, point counts, wire versions 3..5 and compression options.
+ * infos[f] is frame f's whole EncodingInfo; its width * height must equal the frame's point count and the blob's header
+ * states them (width = height = 0: (points, 1)). Blob f is byte-identical to cldn_b200_encoder_create(&infos[f]) +
+ * cldn_b200_encoder_set_dims(w_f, h_f) + cldn_b200_encode(..., write_header = 1), i.e. to that frame's
+ * cldn_b200_encode_blobs alone (with this handle's stage-2 setting).
+ * status[f] (host array, always filled): CLDN_OK or the status that cldn_b200_encoder_create(&infos[f]) followed by that
+ * frame's cldn_b200_encode_blobs returns for that frame alone: a plan this build cannot run, point_step 0, a cloud that
+ * is not a whole number of points, a capacity below the worst case, width * height != points, ZSTD with
+ * CLDN_MEM_DEVICE and no device stage 2, a missing system library. Its message: cldn_b200_mixed_encoder_frame_error(f).
+ * A frame refused on the host writes no byte of its output; the good frames are encoded whatever the others are.
+ * `mem` is one of the three memory kinds, with the routes and refusals of cldn_b200_encode_batch. Frames that share a
+ * layout, compression option and route are encoded by one call of the fused batch path, group after group on the
+ * handle's stream. CLDN_MEM_DEVICE: the encode_batch launches of every group, then one launch that places the headers
+ * of all frames; the blob sizes are read back once, into `written` (optional: with written == NULL the call returns
+ * after enqueueing, and cldn_b200_mixed_encoder_sizes_device holds the sizes once the stream is synchronised).
+ * Host blobs: the call returns with them complete. A group the device fails (never, as the capacities are checked
+ * against the worst case) is encoded again frame by frame, so that only the guilty frame gets the status.
+ * Returns CLDN_OK when every frame was encoded, otherwise the status of the lowest-index failed frame, and
+ * cldn_b200_last_error() reads "frame <f>: <message>". */
+int cldn_b200_encode_mixed_blobs(cldn_mixed_encoder_t* m, size_t n_frames, const cldn_info_t* infos,
+                                 const void* const* clouds, const size_t* cloud_bytes, void* const* outs,
+                                 const size_t* out_capacities, int mem, int32_t* status, size_t* written);
+/* Message of frame f of this handle's last cldn_b200_encode_mixed_blobs ("" when it was encoded). */
+const char* cldn_b200_mixed_encoder_frame_error(const cldn_mixed_encoder_t* m, size_t f);
+/* Device array with one uint64 per frame of the last CLDN_MEM_DEVICE call: the blob size, headers included (0 for a
+ * failed frame). Valid after the stream is synchronised. */
+const uint64_t* cldn_b200_mixed_encoder_sizes_device(const cldn_mixed_encoder_t* m);
+/* Number of layouts whose plans the handle holds now (diagnostics: bounded by 16 or the layouts of the last call). */
+size_t cldn_b200_mixed_encoder_cached_layouts(const cldn_mixed_encoder_t* m);
+/* Waits for everything enqueued on the handle's stream; reports device-side errors of the last call. */
+int cldn_b200_mixed_encoder_sync(cldn_mixed_encoder_t* m);
 
 /* ---- decoder -------------------------------------------------------------------------------------------------- */
 int cldn_b200_decoder_create(int device, void* stream, cldn_decoder_t** out);
