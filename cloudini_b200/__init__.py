@@ -20,7 +20,8 @@ from typing import List, Optional, Sequence
 __all__ = [
     "FieldType", "EncodingOptions", "CompressionOption", "PointField", "EncodingInfo", "EncodingInfoToYAML",
     "EncodingInfoFromYAML", "EncodeHeader", "DecodeHeader", "MaxCompressedSize", "PointcloudEncoder", "MixedEncoder",
-    "PointcloudDecoder", "SizeOf", "lib", "library_path", "kernel_launch_count", "kDecodeButSkipStore",
+    "PointcloudDecoder", "SizeOf", "lib", "library_path", "kernel_launch_count", "kDecodeButSkipStore", "blob_descs",
+    "pack_blob_descs",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -164,6 +165,8 @@ def lib():
                                          C.POINTER(sz), C.c_int, C.c_int]
     L.cldn_b200_decode_blobs.argtypes = [vp, sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(sz), C.c_int,
                                          C.POINTER(C.c_int32), C.POINTER(sz)]
+    L.cldn_b200_decoder_prepare_blobs.argtypes = [vp, C.POINTER(_CInfo), sz, C.c_uint64]
+    L.cldn_b200_decode_blobs_async.argtypes = [vp, sz, vp, vp, vp]
     L.cldn_b200_decoder_frame_error.argtypes = [vp, sz]
     L.cldn_b200_decoder_frame_error.restype = C.c_char_p
     L.cldn_b200_decoder_frame_info.argtypes = [vp, sz, C.POINTER(_CInfo)]
@@ -546,6 +549,28 @@ class MixedEncoder:
         _check(lib().cldn_b200_mixed_encoder_sync(self._h))
 
 
+def blob_descs(descs: Sequence):
+    """numpy uint64 array [n, 4] of cldn_blob_desc_t: one (blob_ptr, blob_bytes, out_ptr, capacity) per frame, all
+    device addresses and sizes as decode_blobs_async() reads them."""
+    import numpy as np
+    a = np.zeros((len(descs), 4), dtype=np.uint64)
+    for f, d in enumerate(descs):
+        a[f] = [int(v) for v in d]
+    return a
+
+
+def pack_blob_descs(descs: Sequence, out=None):
+    """The descriptors of blob_descs() in device memory the caller owns: a new CUDA uint8 tensor, or `out` (a CUDA
+    tensor of at least 32 * len(descs) bytes, e.g. the one a captured graph reads) overwritten on torch's current stream.
+    Returns the tensor; its data_ptr() is decode_blobs_async()'s frames_ptr."""
+    import torch
+    host = torch.from_numpy(blob_descs(descs).view("uint8").reshape(-1))
+    if out is None:
+        return host.cuda()
+    out.view(torch.uint8).reshape(-1)[:host.numel()].copy_(host)
+    return out
+
+
 class PointcloudDecoder:
     """Cloudini::PointcloudDecoder (cloudini.hpp:216-244) backed by the sm_90a kernels."""
 
@@ -656,6 +681,20 @@ class PointcloudDecoder:
                         (C.c_void_p * m)(*out_ptrs), (C.c_size_t * m)(*out_caps), MEM_DEVICE_POINTS)
         del ins
         return r
+
+    def prepare_blobs(self, info: EncodingInfo, max_frames: int, max_points: int):
+        """Prepares decode_blobs_async() for blobs of `info`'s layout (width / height ignored): at most `max_frames`
+        frames of at most `max_points` points each per call. Call it outside any CUDA graph capture; it replaces the
+        previous prepared layout (graphs captured before are then invalid), and leaves the other calls' state alone."""
+        c = _to_c(info)
+        _check(lib().cldn_b200_decoder_prepare_blobs(self._h, C.byref(c), max_frames, max_points))
+
+    def decode_blobs_async(self, frames_ptr: int, n: int, status_ptr: int, decoded_ptr: int = 0):
+        """Enqueues the decode of n device-resident blobs of the prepared layout on this decoder's stream and returns.
+        frames_ptr: device address of n descriptors (pack_blob_descs); status_ptr: device int32[n]; decoded_ptr
+        (optional): device uint64[n]. Statuses are valid once the stream is synchronised; there are no messages (decode a
+        failed blob with decode_blobs_device for its message). The call can be captured in a CUDA graph."""
+        _check(lib().cldn_b200_decode_blobs_async(self._h, n, frames_ptr or None, status_ptr or None, decoded_ptr or None))
 
     def frame_error(self, f: int) -> str:
         """Message of frame f of the last decode_blobs / decode_blobs_device ("" when it decoded)."""

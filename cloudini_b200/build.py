@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libcloudini_b200.so")
 SOURCES = ["cldn_host.cpp", "cldn_ros.cpp", "cldn_encode.cu", "cldn_decode.cu", "cldn_decode_tiles.cu", "cldn_sections.cu", "cldn_preproc.cu", "cldn_lz4.cu", "cldn_zstd.cu",
-           "cldn_zstd_enc.cu", "cldn_api.cu"]
+           "cldn_zstd_enc.cu", "cldn_blobs_async.cu", "cldn_api.cu"]
 HEADERS = ["cldn_plan.h", "cldn_kernels.h", "cldn_device.cuh", "cldn_stage2.cuh", "cldn_decode_fast.cuh", "cldn_encode_fast.cuh", "cldn_encode_points.cuh", "../../include/cloudini_b200.h", "../../include/cloudini_b200_ros.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

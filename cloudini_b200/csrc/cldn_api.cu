@@ -1033,6 +1033,44 @@ int cldn_b200_encode_blobs(cldn_encoder_t* e, size_t n_frames, const void* const
 }  // extern "C"
 
 // =====================================================================================================================
+// The device scratch of the stage-1 decode kernels (DecLaunch). A decoder has one for its calls, and one more for the
+// shape that cldn_b200_decoder_prepare_blobs sized, so that neither invalidates the other.
+struct DecStage1 {
+  DevBuf<uint64_t> d_chunk_offsets;
+  DevBuf<uint32_t> d_chunk_sizes;
+  DevBuf<uint32_t> d_chunk_tiles, d_chunk_tile_begin, d_stream_end, d_tsums, d_chunk_frame, d_tile_chunk;
+  DevBuf<uint64_t> d_tstatus;
+  DevBuf<uint32_t> d_counter, d_redo;
+  DevBuf<uint8_t> d_side;         // side mode: section values decoded ahead of the regular stream (DecLaunch::side)
+  DevBuf<uint64_t> d_chunk_desc;  // chunk-sequential kernel: self-validating chunk descriptors (see walk_frame_publish)
+  uint32_t desc_tag = 0;
+  uint32_t epoch = 0;
+  // the last launch of this scratch (cldn_b200_decoder_last_stats / _last_sections_ahead read the handle's own)
+  bool fast_launched = false;  // it went through decode_floatn_fast_kernel
+  uint32_t fast_chunks = 0;
+  bool sections_ahead = false;  // it ran in side mode
+};
+
+// What the host knows about the frames of one stage-1 launch.
+struct Stage1Shape {
+  uint32_t n_frames = 0;
+  uint64_t chunks = 0;          // chunk slots
+  uint64_t tiles = 0;           // bound of the FloatN tiles of the launch (tile-parallel kernel)
+  uint32_t uniform_chunks = 0;  // > 0: every frame has this many chunk slots
+  // The launch may be replayed from a CUDA graph, with the same tag and epoch every time: the chunk descriptors and the
+  // tile records are cleared in the launch instead of being told apart by a new tag / epoch per call.
+  bool replayable = false;
+  bool empty_slots = false;     // frames own fixed chunk slots, some of them empty (DecLaunch::empty_slots)
+  uint64_t chunk_bytes_max = 0;  // > 0: `tiles` assumes chunk bodies of at most this many bytes (DecLaunch::chunk_bytes_max)
+};
+
+struct cldn_decoder;
+static int launch_stage1(cldn_decoder* d, DecStage1& s, const Plan& plan, const Plan* d_plan, const DecFrame* d_frames,
+                         const Stage1Shape& shape, uint32_t* err, uint32_t* frame_err, bool reserve_only);
+
+struct AsyncBlobs;  // cldn_b200_decoder_prepare_blobs
+struct AsyncBlobsDeleter { void operator()(AsyncBlobs* a) const; };
+
 struct cldn_decoder {
   std::vector<uint8_t> s2_tmp;  // stage-2 decompression scratch (host-pointer API only)
   int device = 0;
@@ -1045,17 +1083,10 @@ struct cldn_decoder {
   DevBuf<Plan> d_plan;
   DevBuf<DecFrame> d_frames;
   PinRing<DecFrame> h_frames;
-  DevBuf<uint64_t> d_chunk_offsets;
-  DevBuf<uint32_t> d_chunk_sizes;
   DevBuf<uint32_t> d_err;
   PinBuf<uint32_t> h_err;
   DevBuf<uint8_t> d_in, d_out;
-  DevBuf<uint32_t> d_chunk_tiles, d_chunk_tile_begin, d_stream_end, d_tsums, d_chunk_frame, d_tile_chunk;
-  DevBuf<uint64_t> d_tstatus;
-  DevBuf<uint32_t> d_counter, d_redo;
-  DevBuf<uint8_t> d_side;         // side mode: section values decoded ahead of the regular stream (DecLaunch::side)
-  DevBuf<uint64_t> d_chunk_desc;  // chunk-sequential kernel: self-validating chunk descriptors (see walk_frame_publish)
-  uint32_t desc_tag = 0;
+  DecStage1 s1;
   // stage 2 on the device (LZ4)
   DevBuf<uint8_t> d_s1, d_lz_scratch;
   DevBuf<uint32_t> d_lz_chunk_frame, d_lz_chunk_sizes;
@@ -1065,11 +1096,7 @@ struct cldn_decoder {
   PinRing<Lz4Frame> h_lz_frames;
   PinRing<uint32_t> h_lz_chunk_frame;
   DevBuf<uint8_t> d_zs_lit;        // ZSTD: literal scratch per decompressing warp
-  bool fast_launched = false;  // the last batch went through decode_floatn_fast_kernel (cldn_b200_decoder_last_stats)
-  uint32_t fast_chunks = 0;
-  bool sections_ahead = false;    // the last batch ran in side mode (cldn_b200_decoder_last_sections_ahead)
   CopyPipeline pipe;
-  uint32_t epoch = 0;
   // cldn_b200_decode_blobs: the first bytes of device-resident blobs, and what the last call found for every frame
   DevBuf<uint64_t> d_blob_tab;
   PinBuf<uint64_t> h_blob_tab;
@@ -1081,6 +1108,7 @@ struct cldn_decoder {
   uint32_t* frame_err = nullptr;
   std::vector<std::string> frame_errors;
   std::vector<cldn_info_t> frame_infos;
+  std::unique_ptr<AsyncBlobs, AsyncBlobsDeleter> async;  // cldn_b200_decoder_prepare_blobs
 };
 
 static bool same_fields(const cldn_info_t& a, const cldn_info_t& b) {
@@ -1098,12 +1126,10 @@ static bool same_info(const cldn_info_t& a, const cldn_info_t& b) {
   return a.width == b.width && a.height == b.height && same_fields(a, b);
 }
 
-// PointcloudDecoder::updateDecoders (cloudini.cpp:627-633)
-static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
-  if (d->have_plan && same_info(d->info, info)) return CLDN_OK;
-  Plan plan;
-  if (int rc = build_decode_plan(info, &plan)) return rc;
-  if (!plan.supported) {
+// The stage-1 decoder plan of `info` (compression NONE), or the refusal.
+static int make_decode_plan(const cldn_info_t& info, Plan* plan) {
+  if (int rc = build_decode_plan(info, plan)) return rc;
+  if (!plan->supported) {
     set_error("EncodingInfo contains a field decoder this build cannot run");
     return CLDN_ERR_UNSUPPORTED;
   }
@@ -1112,6 +1138,14 @@ static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
     return CLDN_ERR_UNSUPPORTED;
   }
   if (info.version < 3) { set_error("wire version %d (single unframed chunk) is not supported", info.version); return CLDN_ERR_UNSUPPORTED; }
+  return CLDN_OK;
+}
+
+// PointcloudDecoder::updateDecoders (cloudini.cpp:627-633)
+static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
+  if (d->have_plan && same_info(d->info, info)) return CLDN_OK;
+  Plan plan;
+  if (int rc = make_decode_plan(info, &plan)) return rc;
   if (int rc = d->d_plan.reserve(1)) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->d_plan.p, &plan, sizeof(Plan), cudaMemcpyHostToDevice, d->stream));
   CUDA_TRY(cudaStreamSynchronize(d->stream));  // `plan` is a stack object
@@ -1142,7 +1176,7 @@ static int decoder_update_plan(cldn_decoder* d, const cldn_info_t& info) {
 static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t n_frames, const void* const* payloads,
                                const size_t* payload_bytes, void* const* outs, const size_t* out_capacities,
                                const uint64_t* frame_points) {
-  d->sections_ahead = false;
+  d->s1.sections_ahead = false;
   if (int rc = decoder_update_plan(d, info)) return rc;
   const uint64_t wh = static_cast<uint64_t>(info.width) * info.height;
   for (size_t f = 0; f < (frame_points ? n_frames : 1); ++f) {
@@ -1171,95 +1205,117 @@ static int decode_batch_device(cldn_decoder* d, const cldn_info_t& info, size_t 
     chunks += F.n_chunks;
   }
   if (chunks > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-  if (int rc = d->d_chunk_offsets.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-  if (int rc = d->d_chunk_sizes.reserve(static_cast<size_t>(chunks) + 1)) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->d_frames.p, hf, n_frames * sizeof(DecFrame), cudaMemcpyHostToDevice, d->stream));
   if (int rc = d->h_frames.commit(hf_slot, d->stream)) return rc;
+  Stage1Shape shape;
+  shape.n_frames = static_cast<uint32_t>(n_frames);
+  shape.chunks = chunks;
+  // tile-parallel path: every chunk adds at most 2 tiles of rounding / misalignment
+  for (size_t f = 0; f < n_frames; ++f) shape.tiles += payload_bytes[f] / decode_tile_bytes() + 2ull * hf[f].n_chunks + 1;
+  bool uniform = n_frames > 0 && hf[0].n_chunks > 0;
+  for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
+  shape.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
+  return launch_stage1(d, d->s1, d->plan, d->d_plan.p, d->d_frames.p, shape, d->d_err.p, d->frame_err, false);
+}
+
+// The stage-1 kernels of one launch, routed by the plan and the host's view of the frames (`shape`); the frame table is on
+// the device. reserve_only: size the scratch of this shape and launch nothing.
+static int launch_stage1(cldn_decoder* d, DecStage1& s, const Plan& plan, const Plan* d_plan, const DecFrame* d_frames,
+                         const Stage1Shape& shape, uint32_t* err, uint32_t* frame_err, bool reserve_only) {
+  const uint64_t chunks = shape.chunks;
+  if (int rc = s.d_chunk_offsets.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+  if (int rc = s.d_chunk_sizes.reserve(static_cast<size_t>(chunks) + 1)) return rc;
   DecLaunch L{};
-  L.frames = d->d_frames.p;
-  L.n_frames = static_cast<uint32_t>(n_frames);
+  L.frames = d_frames;
+  L.n_frames = shape.n_frames;
   L.n_chunks_total = static_cast<uint32_t>(chunks);
-  L.plan = d->d_plan.p;
-  L.chunk_offsets = d->d_chunk_offsets.p;
-  L.chunk_sizes = d->d_chunk_sizes.p;
-  L.err = d->d_err.p;
-  L.frame_err = d->frame_err;
-  if (d->plan.n_sections > 0 && chunks > 0 && (d->plan.regular_overlap || !(d->plan.all_varint || d->plan.n_ops == 0))) {
+  L.plan = d_plan;
+  L.chunk_offsets = s.d_chunk_offsets.p;
+  L.chunk_sizes = s.d_chunk_sizes.p;
+  L.err = err;
+  L.frame_err = frame_err;
+  L.empty_slots = shape.empty_slots ? 1u : 0u;
+  if (plan.n_sections > 0 && chunks > 0 && (plan.regular_overlap || !(plan.all_varint || plan.n_ops == 0))) {
     // V5 with raw / XOR / Gorilla fields in the regular stream: the per-chunk parser records where the sections start
-    if (int rc = d->d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    L.stream_end = d->d_stream_end.p;
+    if (int rc = s.d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    L.stream_end = s.d_stream_end.p;
   }
   const char* force_env = getenv("CLDN_B200_FORCE_CHUNK_DECODE");
   const bool force_chunk = force_env && force_env[0] == '1';
-  const bool fast_general = !d->plan.floatn_only && chunks > 0 && decode_fast_general_plan(d->plan) &&
+  const bool fast_general = !plan.floatn_only && chunks > 0 && decode_fast_general_plan(plan) &&
                             decode_tiles_sequential(static_cast<uint32_t>(chunks)) && decode_fast_enabled() && !force_chunk;
-  const bool tile_parallel = d->plan.floatn_only && chunks > 0 && !force_chunk;
+  const bool tile_parallel = plan.floatn_only && chunks > 0 && !force_chunk;
   if (fast_general) {
     // float-varint streams with scalar lossy fields (Velodyne XYZIRT ...): fast chunk-sequential reader + redo list
-    if (int rc = d->d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    L.stream_end = d->d_stream_end.p;
+    if (int rc = s.d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    L.stream_end = s.d_stream_end.p;
   }
   if (tile_parallel) {
-    // tile-parallel path: host upper bound on the tile count (every chunk adds at most 2 tiles of rounding/misalignment)
-    uint64_t tiles = 0;
-    for (size_t f = 0; f < n_frames; ++f) tiles += payload_bytes[f] / decode_tile_bytes() + 2ull * hf[f].n_chunks + 1;
+    const uint64_t tiles = shape.tiles;
     if (tiles > 0x7FFFFFFFull) { set_error("batch too large"); return CLDN_ERR_UNSUPPORTED; }
-    if (int rc = d->d_chunk_tiles.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    if (int rc = d->d_chunk_tile_begin.reserve(static_cast<size_t>(chunks) + 2)) return rc;
-    if (int rc = d->d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    if (int rc = d->d_chunk_frame.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    if (int rc = d->d_tile_chunk.reserve(static_cast<size_t>(tiles) + 1)) return rc;
-    const size_t old_cap = d->d_tstatus.cap;
-    if (int rc = d->d_tstatus.reserve(static_cast<size_t>(tiles) + 1, true)) return rc;
-    if (d->d_tstatus.cap != old_cap || d->d_tsums.cap < d->d_tstatus.cap * 16) {
-      if (int rc = d->d_tsums.reserve(d->d_tstatus.cap * 16, true)) return rc;
+    if (int rc = s.d_chunk_tiles.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    if (int rc = s.d_chunk_tile_begin.reserve(static_cast<size_t>(chunks) + 2)) return rc;
+    if (int rc = s.d_stream_end.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    if (int rc = s.d_chunk_frame.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    if (int rc = s.d_tile_chunk.reserve(static_cast<size_t>(tiles) + 1)) return rc;
+    const size_t old_cap = s.d_tstatus.cap;
+    if (int rc = s.d_tstatus.reserve(static_cast<size_t>(tiles) + 1, true)) return rc;
+    if (s.d_tstatus.cap != old_cap || s.d_tsums.cap < s.d_tstatus.cap * 16) {
+      if (int rc = s.d_tsums.reserve(s.d_tstatus.cap * 16, true)) return rc;
     }
-    d->epoch = (d->epoch + 1) & 0x3FFFFFu;
-    if (d->epoch == 0) {
-      CUDA_TRY(cudaMemsetAsync(d->d_tstatus.p, 0, d->d_tstatus.cap * sizeof(uint64_t), d->stream));
-      CUDA_TRY(cudaMemsetAsync(d->d_tsums.p, 0, d->d_tsums.cap * sizeof(uint32_t), d->stream));
-      d->epoch = 1;
+    // a replayable launch clears the records it will read: none on the chunk-sequential route, which has no tile records
+    const bool clear = shape.replayable && !decode_tiles_sequential(static_cast<uint32_t>(chunks));
+    if (!reserve_only) {
+      s.epoch = shape.replayable ? 1u : (s.epoch + 1) & 0x3FFFFFu;
+      if (s.epoch == 0 || clear) {
+        CUDA_TRY(cudaMemsetAsync(s.d_tstatus.p, 0, (shape.replayable ? tiles + 1 : s.d_tstatus.cap) * sizeof(uint64_t), d->stream));
+        CUDA_TRY(cudaMemsetAsync(s.d_tsums.p, 0, (shape.replayable ? 16 * (tiles + 1) : s.d_tsums.cap) * sizeof(uint32_t), d->stream));
+        if (s.epoch == 0) s.epoch = 1;
+      }
     }
-    L.chunk_tiles = d->d_chunk_tiles.p;
-    L.chunk_tile_begin = d->d_chunk_tile_begin.p;
-    L.stream_end = d->d_stream_end.p;
-    L.chunk_frame = d->d_chunk_frame.p;
-    L.tile_chunk = d->d_tile_chunk.p;
-    L.tstatus = d->d_tstatus.p;
-    L.tsums = d->d_tsums.p;
-    L.tile_capacity = static_cast<uint32_t>(d->d_tstatus.cap);
+    L.chunk_tiles = s.d_chunk_tiles.p;
+    L.chunk_tile_begin = s.d_chunk_tile_begin.p;
+    L.stream_end = s.d_stream_end.p;
+    L.chunk_frame = s.d_chunk_frame.p;
+    L.tile_chunk = s.d_tile_chunk.p;
+    L.tstatus = s.d_tstatus.p;
+    L.tsums = s.d_tsums.p;
+    L.tile_capacity = static_cast<uint32_t>(s.d_tstatus.cap);
     L.tile_grid = static_cast<uint32_t>(tiles);
-    L.epoch = d->epoch;
+    L.chunk_bytes_max = static_cast<uint32_t>(shape.chunk_bytes_max);
+    L.epoch = s.epoch;
   }
   if (fast_general || tile_parallel) {
     // chunk claim counters, the careful kernel's redo list and the self-validating chunk descriptors
-    if (int rc = d->d_counter.reserve(4, true)) return rc;
-    if (int rc = d->d_redo.reserve(static_cast<size_t>(chunks) + 1)) return rc;
-    const size_t had = d->d_chunk_desc.cap;
-    if (int rc = d->d_chunk_desc.reserve(2 * static_cast<size_t>(chunks) + 2)) return rc;
-    d->desc_tag = (d->desc_tag + 1) & 0xFFFFFFu;
-    if (d->d_chunk_desc.cap != had || d->desc_tag == 0) {  // fresh memory or tag wrap: no stale word may carry a live tag
-      CUDA_TRY(cudaMemsetAsync(d->d_chunk_desc.p, 0, d->d_chunk_desc.cap * sizeof(uint64_t), d->stream));
-      if (d->desc_tag == 0) d->desc_tag = 1;
+    if (int rc = s.d_counter.reserve(4, true)) return rc;
+    if (int rc = s.d_redo.reserve(static_cast<size_t>(chunks) + 1)) return rc;
+    const size_t had = s.d_chunk_desc.cap;
+    if (int rc = s.d_chunk_desc.reserve(2 * static_cast<size_t>(chunks) + 2)) return rc;
+    if (!reserve_only) {
+      s.desc_tag = shape.replayable ? 1u : (s.desc_tag + 1) & 0xFFFFFFu;
+      if (s.d_chunk_desc.cap != had || s.desc_tag == 0 || shape.replayable) {  // fresh memory, tag wrap or replay: no stale word may carry a live tag
+        CUDA_TRY(cudaMemsetAsync(s.d_chunk_desc.p, 0, (shape.replayable ? 2 * chunks + 2 : s.d_chunk_desc.cap) * sizeof(uint64_t), d->stream));
+        if (s.desc_tag == 0) s.desc_tag = 1;
+      }
     }
-    L.chunk_counter = d->d_counter.p;
-    L.redo_list = d->d_redo.p;
-    L.chunk_desc = d->d_chunk_desc.p;
-    L.desc_tag = d->desc_tag;
-    bool uniform = n_frames > 0 && hf[0].n_chunks > 0;
-    for (size_t f = 1; f < n_frames; ++f) uniform = uniform && hf[f].n_chunks == hf[0].n_chunks;
-    L.uniform_chunks = uniform ? hf[0].n_chunks : 0u;
+    L.chunk_counter = s.d_counter.p;
+    L.redo_list = s.d_redo.p;
+    L.chunk_desc = s.d_chunk_desc.p;
+    L.desc_tag = s.desc_tag;
+    L.uniform_chunks = shape.uniform_chunks;
   }
-  d->fast_launched = L.redo_list != nullptr && decode_tiles_sequential(L.n_chunks_total) && decode_fast_enabled() && !d->plan.regular_overlap;
-  if (d->fast_launched && L.chunk_desc && L.stream_end && L.chunk_counter && decode_side_plan(d->plan) && decode_fast_general_plan(d->plan) && !force_chunk) {
+  const bool fast_launched = L.redo_list != nullptr && decode_tiles_sequential(L.n_chunks_total) && decode_fast_enabled() && !plan.regular_overlap;
+  if (fast_launched && L.chunk_desc && L.stream_end && L.chunk_counter && decode_side_plan(plan) && decode_fast_general_plan(plan) && !force_chunk) {
     // V5 sections ahead of the regular stream: compact per-chunk arrays the fast reader merges into the rows (DecLaunch::side)
-    const size_t side_bytes = decode_side_bytes(d->plan, chunks, L.side_off);
-    if (int rc = d->d_side.reserve(side_bytes + 256)) return rc;
-    L.side = d->d_side.p;
+    const size_t side_bytes = decode_side_bytes(plan, chunks, L.side_off);
+    if (int rc = s.d_side.reserve(side_bytes + 256)) return rc;
+    L.side = s.d_side.p;
   }
-  d->sections_ahead = decode_side_active(d->plan, L);
-  d->fast_chunks = d->fast_launched ? L.n_chunks_total : 0u;
-  if (launch_decode(d->plan, L, d->stream) < 0) { set_error("decode kernel launch failed"); return CLDN_ERR_CUDA; }
+  if (reserve_only) return CLDN_OK;
+  s.fast_launched = fast_launched;
+  s.sections_ahead = decode_side_active(plan, L);
+  s.fast_chunks = fast_launched ? L.n_chunks_total : 0u;
+  if (launch_decode(plan, L, d->stream) < 0) { set_error("decode kernel launch failed"); return CLDN_ERR_CUDA; }
   CUDA_TRY(cudaGetLastError());
   return CLDN_OK;
 }
@@ -1308,18 +1364,18 @@ int cldn_b200_decoder_last_stats(cldn_decoder_t* d, uint32_t stats[2]) {
   if (!d || !stats) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
   stats[0] = stats[1] = 0;
   CUDA_TRY(cudaSetDevice(d->device));
-  if (!d->d_counter.p || !d->fast_launched) return CLDN_OK;
+  if (!d->s1.d_counter.p || !d->s1.fast_launched) return CLDN_OK;
   uint32_t c[4] = {0, 0, 0, 0};
   CUDA_TRY(cudaStreamSynchronize(d->stream));
-  CUDA_TRY(cudaMemcpy(c, d->d_counter.p, sizeof(c), cudaMemcpyDeviceToHost));
-  stats[0] = d->fast_chunks;
+  CUDA_TRY(cudaMemcpy(c, d->s1.d_counter.p, sizeof(c), cudaMemcpyDeviceToHost));
+  stats[0] = d->s1.fast_chunks;
   stats[1] = c[3];
   return CLDN_OK;
 }
 
 int cldn_b200_decoder_last_sections_ahead(cldn_decoder_t* d) {
   if (!d) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
-  return d->sections_ahead ? 1 : 0;
+  return d->s1.sections_ahead ? 1 : 0;
 }
 
 }  // extern "C"
@@ -1370,6 +1426,29 @@ static bool zstd_host_route() {
   return v && v[0] == '1';
 }
 
+// The stage-2 kernels of one launch: every chunk of L is decompressed into its slot, LZ4 or ZSTD (`zstd`, into at most
+// body_cap bytes), and the slots are re-framed into one stage-1 payload per frame (sizes in L.sizes). reserve_only: size
+// the ZSTD literal scratch `lit` and launch nothing.
+static int launch_stage2(cudaStream_t stream, bool zstd, const Lz4Launch& L, size_t body_cap, DevBuf<uint8_t>& lit, bool reserve_only) {
+  if (zstd) {
+    // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
+    const uint32_t wpc = zstd_warps_per_cta();
+    const size_t ctas = std::max<size_t>(1, std::min<size_t>((L.n_chunks_total + wpc - 1) / wpc, 2048 / wpc));
+    if (int rc = lit.reserve(ctas * wpc * zstd_lit_scratch_bytes(static_cast<uint32_t>(body_cap)))) return rc;
+    if (reserve_only) return CLDN_OK;
+    ZstdLaunch Z{};
+    Z.L = L;
+    Z.body_cap = static_cast<uint32_t>(body_cap);
+    Z.n_ctas = static_cast<uint32_t>(ctas);
+    Z.lit_scratch = lit.p;
+    if (launch_zstd_decompress(Z, stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  } else if (!reserve_only && launch_lz4_decompress(L, stream) < 0) {
+    set_error("LZ4 kernel launch failed");
+    return CLDN_ERR_CUDA;
+  }
+  return CLDN_OK;
+}
+
 // Stage 2 on the device, LZ4 or ZSTD (info.compression_opt): every chunk is decompressed into a slot (cldn_lz4.cu,
 // cldn_zstd.cu) and the slots are re-framed into one stage-1 payload per frame in the decoder's arena. On return p1 / b1
 // are those payloads, behind one read-back of their sizes (8 bytes per frame) and one synchronisation. A slot holds the
@@ -1404,15 +1483,8 @@ static int stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_fram
   for (size_t f = 0; zstd && f < n_frames; ++f) {  // a frame without points has no chunk to decompress
     if (fc.frame_chunks(f) == 0 && payload_bytes[f] != 0) { set_error("%s", dev_error_text(DEV_ERR_CHUNK_COUNT)); return CLDN_ERR_CORRUPT_DATA; }
   }
-  size_t ctas = 0, lit_bytes = 0;
-  if (zstd) {  // one warp per chunk up to 2048 warps (literal scratch: <= 128 KB each), then a grid stride
-    const uint32_t wpc = zstd_warps_per_cta();
-    ctas = std::max<size_t>(1, std::min<size_t>((chunks + wpc - 1) / wpc, 2048 / wpc));
-    lit_bytes = ctas * wpc * zstd_lit_scratch_bytes(static_cast<uint32_t>(body_cap));
-  }
   if (int rc = d->d_s1.reserve(std::max<size_t>(fc.arena, 256))) return rc;
   if (int rc = d->d_lz_scratch.reserve(std::max<size_t>(chunks, 1) * slot)) return rc;
-  if (int rc = zstd ? d->d_zs_lit.reserve(lit_bytes) : CLDN_OK) return rc;
   if (int rc = d->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
   if (int rc = d->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
   if (int rc = d->d_lz_frames.reserve(n_frames)) return rc;
@@ -1450,17 +1522,7 @@ static int stage2_device(cldn_decoder* d, const cldn_info_t& info, size_t n_fram
   L.sizes = d->d_lz_sizes.p;
   L.err = d->d_err.p;
   L.frame_err = d->frame_err;
-  if (zstd) {
-    ZstdLaunch Z{};
-    Z.L = L;
-    Z.body_cap = static_cast<uint32_t>(body_cap);
-    Z.n_ctas = static_cast<uint32_t>(ctas);
-    Z.lit_scratch = d->d_zs_lit.p;
-    if (launch_zstd_decompress(Z, d->stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
-  } else if (launch_lz4_decompress(L, d->stream) < 0) {
-    set_error("LZ4 kernel launch failed");
-    return CLDN_ERR_CUDA;
-  }
+  if (int rc = launch_stage2(d->stream, zstd, L, body_cap, d->d_zs_lit, false)) return rc;
   CUDA_TRY(cudaMemcpyAsync(d->h_lz_sizes.p, d->d_lz_sizes.p, n_frames * sizeof(uint64_t), cudaMemcpyDeviceToHost, d->stream));
   if (int rc = check_device_error(d->stream, d->d_err.p, d->h_err.p)) return rc;  // synchronises; damaged frames stop here
   p1.resize(n_frames);
@@ -1861,6 +1923,181 @@ static int decode_blobs_impl(cldn_decoder* d, size_t n, const void* const* blobs
   return result();
 }
 
+// ---- complete device blobs of one prepared layout, without the host (cldn_b200_decode_blobs_async) ------------------
+// Everything the calls of one prepared layout and shape read: uploaded and allocated once by
+// cldn_b200_decoder_prepare_blobs, apart from the buffers of the handle's other calls, so that a call allocates, copies
+// from the host and synchronises nothing, and a CUDA graph that captured one stays valid until the next prepare.
+struct AsyncBlobs {
+  cldn_info_t info;       // the layout as its header states it, width = height = 0
+  Plan plan;              // stage 1 (compression NONE)
+  size_t max_frames = 0;
+  uint32_t slots = 0;     // chunk slots per frame: those of max_points
+  uint64_t tiles_per_frame = 0;
+  uint64_t chunk_bytes_max = 0;  // the chunk bodies the tile grid is sized for
+  size_t body_cap = 0;    // stage 2: bytes a chunk may decompress to
+  DevBuf<Plan> d_plan;
+  DevBuf<uint8_t> d_tmpl;
+  DevBuf<DecFrame> d_frames;
+  DevBuf<Lz4Frame> d_lz_frames;
+  DevBuf<uint32_t> d_lz_chunk_frame, d_lz_chunk_sizes;
+  DevBuf<uint64_t> d_lz_sizes;
+  DevBuf<uint8_t> d_s1, d_lz_scratch, d_zs_lit;
+  DevBuf<uint32_t> d_frame_err, d_err;
+  DecStage1 s1;
+  AsyncLaunch A{};  // all but the call's arrays
+  Lz4Launch Z{};    // all but the call's counts
+
+  // every call launches the grids of max_frames frames: the frames past its own are empty
+  Stage1Shape shape() const {
+    Stage1Shape s;
+    s.n_frames = static_cast<uint32_t>(max_frames);
+    s.chunks = static_cast<uint64_t>(max_frames) * slots;
+    s.tiles = static_cast<uint64_t>(max_frames) * tiles_per_frame;
+    s.chunk_bytes_max = chunk_bytes_max;
+    s.uniform_chunks = slots;
+    s.replayable = true;
+    s.empty_slots = true;
+    return s;
+  }
+};
+void AsyncBlobsDeleter::operator()(AsyncBlobs* a) const { delete a; }
+
+static int prepare_blobs_impl(cldn_decoder* d, const cldn_info_t* layout, size_t max_frames, uint64_t max_points) {
+  if (!d || !layout) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_frames == 0 || max_frames > 0x7FFFFFFFull) { set_error("max_frames must be 1 .. 2^31 - 1"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_points > 0xFFFFFFFFull) { set_error("max_points_per_frame must be below 2^32"); return CLDN_ERR_UNSUPPORTED; }
+  if (layout->version < 3 || layout->version > CLDN_ENCODING_VERSION) {
+    set_error("wire version %d: cldn_b200_decode_blobs_async decodes versions 3 .. %d", layout->version, CLDN_ENCODING_VERSION);
+    return CLDN_ERR_UNSUPPORTED;
+  }
+  if (layout->compression_opt > CLDN_COMP_ZSTD) { set_error("Unsupported compression option"); return CLDN_ERR_INVALID_ARGUMENT; }
+  CUDA_TRY(cudaSetDevice(d->device));
+  CUDA_TRY(cudaStreamSynchronize(d->stream));  // kernels of an earlier prepared state may still read it
+  d->async.reset();
+  std::unique_ptr<AsyncBlobs, AsyncBlobsDeleter> a(new AsyncBlobs());
+  // the header every blob of the layout starts with, and the layout decode_blobs reads from it
+  cldn_info_t zero = *layout;
+  zero.width = zero.height = 0;
+  const std::vector<uint8_t> hdr = make_header(zero);
+  size_t used = 0;
+  if (int rc = cldn_b200_decode_header(hdr.data(), hdr.size(), &a->info, &used)) return rc;
+  const std::string text(reinterpret_cast<const char*>(hdr.data()), hdr.size());
+  const size_t w_at = text.find("\nwidth: 0\nheight: 0\n");
+  if (w_at == std::string::npos) { set_error("the layout's header has no width / height lines"); return CLDN_ERR_INTERNAL; }
+  const uint32_t len0 = static_cast<uint32_t>(w_at + 8), len1 = 9, len2 = static_cast<uint32_t>(hdr.size() - (w_at + 19));
+  std::vector<uint8_t> tmpl(hdr.begin(), hdr.begin() + len0);
+  tmpl.insert(tmpl.end(), hdr.begin() + len0 + 1, hdr.begin() + len0 + 1 + len1);
+  tmpl.insert(tmpl.end(), hdr.begin() + w_at + 19, hdr.end());
+  cldn_info_t plain = a->info;
+  plain.compression_opt = CLDN_COMP_NONE;
+  if (int rc = make_decode_plan(plain, &a->plan)) return rc;
+  const bool compressed = a->info.compression_opt != CLDN_COMP_NONE;
+  a->max_frames = max_frames;
+  a->slots = static_cast<uint32_t>((max_points + kChunkPoints - 1) / kChunkPoints);
+  const uint64_t chunks = static_cast<uint64_t>(max_frames) * a->slots;
+  if (chunks > 0x7FFFFFFFull) { set_error("max_frames * chunks per frame must be below 2^31"); return CLDN_ERR_UNSUPPORTED; }
+  // stage-1 worst case of a chunk of p > 0 points: chunk_a + chunk_b * p (MaxCompressedSize of one chunk)
+  bool ok1, ok2;
+  const size_t m1 = max_compressed_size(plain, 1, false, &ok1), m2 = max_compressed_size(plain, 2, false, &ok2);
+  if (!ok1 || !ok2) return CLDN_ERR_INVALID_ARGUMENT;
+  const uint64_t chunk_b = m2 - m1, chunk_a = m1 - chunk_b;
+  const uint64_t pc = std::min<uint64_t>(max_points, kChunkPoints);
+  a->body_cap = pc ? chunk_a + chunk_b * pc + 64 : 64;  // stage2_device's bound for chunks of pc points
+  const size_t slot = (a->body_cap + 15) & ~size_t(15);
+  const uint64_t s1_stride = (a->slots * (slot + 4) + 255) & ~uint64_t(255);
+  // bound of a chunk's stage-1 bytes for the tile grid: the worst case, with room for the V5 modes that exceed it (one
+  // byte per value of a section and 16 more); a larger chunk, which no encoder writes, fails its frame alone
+  const uint64_t chunk_bound = (pc ? chunk_a + chunk_b * pc : 0) + (pc + 16) * (a->plan.n_sections + 1) + 128;
+  if (chunk_bound > 0xFFFFFFFFull) { set_error("prepared shape too large"); return CLDN_ERR_UNSUPPORTED; }
+  a->chunk_bytes_max = chunk_bound;
+  // a chunk of b bytes spans at most b / tile + 2 tiles (rounding and misalignment)
+  a->tiles_per_frame = a->slots * (chunk_bound / decode_tile_bytes() + 2) + 1;
+  if (static_cast<uint64_t>(max_frames) * a->tiles_per_frame > 0x7FFFFFFFull) { set_error("prepared shape too large"); return CLDN_ERR_UNSUPPORTED; }
+
+  if (int rc = a->d_plan.reserve(1)) return rc;
+  if (int rc = a->d_tmpl.reserve(tmpl.size())) return rc;
+  CUDA_TRY(cudaMemcpyAsync(a->d_plan.p, &a->plan, sizeof(Plan), cudaMemcpyHostToDevice, d->stream));
+  CUDA_TRY(cudaMemcpyAsync(a->d_tmpl.p, tmpl.data(), tmpl.size(), cudaMemcpyHostToDevice, d->stream));
+  if (int rc = a->d_frames.reserve(max_frames)) return rc;
+  if (int rc = a->d_frame_err.reserve(max_frames)) return rc;
+  if (int rc = a->d_err.reserve(1, true)) return rc;
+  AsyncLaunch& A = a->A;
+  A.tmpl = a->d_tmpl.p;
+  A.tmpl_len[0] = len0;
+  A.tmpl_len[1] = len1;
+  A.tmpl_len[2] = len2;
+  A.max_points = max_points;
+  A.point_step = a->info.point_step;
+  A.slots = a->slots;
+  A.compression = a->info.compression_opt;
+  A.frames = a->d_frames.p;
+  A.chunk_a = chunk_a;
+  A.chunk_b = chunk_b;
+  A.frame_err = a->d_frame_err.p;
+  A.err = a->d_err.p;
+  if (compressed) {
+    // stage 2: the chunk -> frame table is the prepared shape's (slot gc belongs to frame gc / slots)
+    if (int rc = a->d_lz_frames.reserve(max_frames)) return rc;
+    if (int rc = a->d_lz_sizes.reserve(max_frames)) return rc;
+    if (int rc = a->d_lz_chunk_sizes.reserve(chunks + 1)) return rc;
+    if (int rc = a->d_lz_chunk_frame.reserve(chunks + 1)) return rc;
+    if (int rc = a->d_lz_scratch.reserve(std::max<uint64_t>(chunks, 1) * slot)) return rc;
+    if (int rc = a->d_s1.reserve(std::max<uint64_t>(max_frames * s1_stride, 256))) return rc;
+    std::vector<uint32_t> chunk_frame(chunks + 1, 0);
+    for (uint64_t gc = 0; gc < chunks; ++gc) chunk_frame[gc] = static_cast<uint32_t>(gc / a->slots);
+    CUDA_TRY(cudaMemcpyAsync(a->d_lz_chunk_frame.p, chunk_frame.data(), chunk_frame.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
+    Lz4Launch& Z = a->Z;
+    Z.frames = a->d_lz_frames.p;
+    Z.chunk_frame = a->d_lz_chunk_frame.p;
+    Z.scratch = a->d_lz_scratch.p;
+    Z.slot_stride = static_cast<uint32_t>(slot);
+    Z.chunk_sizes = a->d_lz_chunk_sizes.p;
+    Z.sizes = a->d_lz_sizes.p;
+    Z.err = a->d_err.p;
+    Z.frame_err = a->d_frame_err.p;
+    Z.n_frames = static_cast<uint32_t>(max_frames);
+    Z.n_chunks_total = static_cast<uint32_t>(chunks);
+    if (int rc = launch_stage2(d->stream, A.compression == CLDN_COMP_ZSTD, Z, a->body_cap, a->d_zs_lit, true)) return rc;
+    A.lz_frames = a->d_lz_frames.p;
+    A.s1 = a->d_s1.p;
+    A.s1_stride = s1_stride;
+    A.s1_sizes = a->d_lz_sizes.p;
+    A.chunk_sizes = a->d_lz_chunk_sizes.p;
+  }
+  A.n_tables = static_cast<uint32_t>(max_frames);
+  if (int rc = launch_stage1(d, a->s1, a->plan, a->d_plan.p, a->d_frames.p, a->shape(), a->d_err.p, a->d_frame_err.p, true)) return rc;
+  CUDA_TRY(cudaStreamSynchronize(d->stream));  // the uploads read host objects of this function
+  d->async = std::move(a);
+  return CLDN_OK;
+}
+
+// Enqueues only. The launches and their grids are those of the prepared shape, whatever the frames (header kernel,
+// stage 2 + link kernel when compressed, the stage-1 launches of the prepared route, status kernel).
+static int decode_blobs_async_impl(cldn_decoder* d, size_t n, const void* d_frames, int32_t* d_status, uint64_t* d_decoded) {
+  if (!d) { set_error("null decoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  AsyncBlobs* a = d->async.get();
+  if (!a) { set_error("no prepared layout: call cldn_b200_decoder_prepare_blobs first"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n > a->max_frames) { set_error("%zu frames: the layout was prepared for at most %zu", n, a->max_frames); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return CLDN_OK;
+  if (!d_frames || !d_status) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  CUDA_TRY(cudaSetDevice(d->device));
+  AsyncLaunch A = a->A;
+  A.desc = static_cast<const BlobDesc*>(d_frames);
+  A.n_frames = static_cast<uint32_t>(n);
+  A.status = d_status;
+  A.decoded = d_decoded;
+  CUDA_TRY(cudaMemsetAsync(a->d_frame_err.p, 0, a->max_frames * sizeof(uint32_t), d->stream));
+  launch_blobs_async_headers(A, d->stream);
+  if (A.compression != CLDN_COMP_NONE) {
+    if (int rc = launch_stage2(d->stream, A.compression == CLDN_COMP_ZSTD, a->Z, a->body_cap, a->d_zs_lit, false)) return rc;
+    launch_blobs_async_link(A, d->stream);
+  }
+  if (int rc = launch_stage1(d, a->s1, a->plan, a->d_plan.p, a->d_frames.p, a->shape(), a->d_err.p, a->d_frame_err.p, false)) return rc;
+  launch_blobs_async_status(A, d->stream);
+  CUDA_TRY(cudaGetLastError());
+  return CLDN_OK;
+}
+
 extern "C" {
 
 int cldn_b200_decode_batch(cldn_decoder_t* d, const cldn_info_t* info, size_t n_frames, const void* const* payloads,
@@ -1871,6 +2108,14 @@ int cldn_b200_decode_batch(cldn_decoder_t* d, const cldn_info_t* info, size_t n_
 int cldn_b200_decode_blobs(cldn_decoder_t* dec, size_t n_frames, const void* const* blobs, const size_t* blob_bytes,
                            void* const* outs, const size_t* out_capacities, int mem, int32_t* status, size_t* decoded_bytes) {
   return guarded([&] { return decode_blobs_impl(dec, n_frames, blobs, blob_bytes, outs, out_capacities, mem, status, decoded_bytes); });
+}
+
+int cldn_b200_decoder_prepare_blobs(cldn_decoder_t* dec, const cldn_info_t* layout, size_t max_frames, uint64_t max_points_per_frame) {
+  return guarded([&] { return prepare_blobs_impl(dec, layout, max_frames, max_points_per_frame); });
+}
+
+int cldn_b200_decode_blobs_async(cldn_decoder_t* dec, size_t n_frames, const void* d_frames, int32_t* d_status, uint64_t* d_decoded_bytes) {
+  return guarded([&] { return decode_blobs_async_impl(dec, n_frames, d_frames, d_status, d_decoded_bytes); });
 }
 
 const char* cldn_b200_decoder_frame_error(const cldn_decoder_t* dec, size_t f) {

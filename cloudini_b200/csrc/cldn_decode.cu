@@ -835,6 +835,7 @@ __global__ void __launch_bounds__(kThreads) decode_chunks_kernel(const DecLaunch
   }
   __syncthreads();
   const DecFrame F = L.frames[s_frame];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   const uint32_t n_points = min(kChunkPoints, F.n_points - c * kChunkPoints);
   const uint8_t* body = F.payload + L.chunk_offsets[gc];
@@ -896,6 +897,7 @@ __global__ void __launch_bounds__(kThreads) decode_fixed_kernel(const DecLaunch 
     if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
   }
   const DecFrame F = L.frames[lo];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   const uint32_t n_points = min(kChunkPoints, F.n_points - c * kChunkPoints);
   const uint8_t* body = F.payload + L.chunk_offsets[gc];
@@ -930,6 +932,7 @@ __global__ void decode_sequential_kernel(const DecLaunch L) {
     if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
   }
   const DecFrame F = L.frames[lo];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   const uint32_t n_points = min(kChunkPoints, F.n_points - c * kChunkPoints);
   const uint8_t* p = F.payload + L.chunk_offsets[gc];
@@ -1144,6 +1147,7 @@ __global__ void __launch_bounds__(kThreads) decode_mixed_kernel(const DecLaunch 
   }
   __syncthreads();
   const DecFrame F = L.frames[s_frame];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   const uint32_t n_points = min(kChunkPoints, F.n_points - c * kChunkPoints);
   const uint8_t* body = F.payload + L.chunk_offsets[gc];
@@ -1465,6 +1469,7 @@ __global__ void __launch_bounds__(kThreads) decode_gorilla_kernel(const DecLaunc
   }
   __syncthreads();
   const DecFrame F = L.frames[s_frame];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   const uint32_t n_points = min(kChunkPoints, F.n_points - c * kChunkPoints);
   const uint8_t* body = F.payload + L.chunk_offsets[gc];

@@ -159,29 +159,25 @@ __global__ void __launch_bounds__(kFT, kFastDecMinBlocks) decode_floatn_fast_ker
       uint32_t gc_ = i;
       if (i < L.n_chunks_total) {
         if (L.uniform_chunks) gc_ = (i % L.n_frames) * L.uniform_chunks + i / L.n_frames;
-        unsigned long long w0, w1;
-        do {
-          w0 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_);
-          w1 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_ + 1);
-        } while (static_cast<uint32_t>(w0 >> 40) != L.desc_tag || static_cast<uint32_t>(w1 >> 40) != L.desc_tag);
-        sh.desc[0] = w0 & 0xFFFFFFFFFFull;
-        sh.desc[1] = w1 & 0xFFFFFFFFull;
+        if (!L.empty_slots || !chunk_slot_empty(L.frames[dec_frame_of(L, gc_)], gc_)) {  // nobody publishes an empty slot
+          unsigned long long w0, w1;
+          do {
+            w0 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_);
+            w1 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_ + 1);
+          } while (static_cast<uint32_t>(w0 >> 40) != L.desc_tag || static_cast<uint32_t>(w1 >> 40) != L.desc_tag);
+          sh.desc[0] = w0 & 0xFFFFFFFFFFull;
+          sh.desc[1] = w1 & 0xFFFFFFFFull;
+        }
       }
       sh.chunk = gc_;
     }
     __syncthreads();
     const uint32_t gc = sh.chunk;
     if (gc >= L.n_chunks_total) return;
-    uint32_t fidx;
-    if (L.uniform_chunks) {
-      fidx = gc / L.uniform_chunks;
-    } else {
-      uint32_t lo = 0, hi = L.n_frames - 1;
-      while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
-      }
-      fidx = lo;
+    const uint32_t fidx = dec_frame_of(L, gc);
+    if (L.empty_slots && chunk_slot_empty(L.frames[fidx], gc)) {
+      __syncthreads();  // everybody has read sh.chunk before thread 0 may claim the next chunk
+      continue;
     }
     const uint32_t n_points = [&] {
       const DecFrame F = L.frames[fidx];
@@ -818,6 +814,9 @@ __global__ void __launch_bounds__(kSeT) stream_end_kernel(const DecLaunch L, con
   }
   const uint32_t gc = blockIdx.x;
   if (gc >= L.n_chunks_total) return;
+  const uint32_t fidx = dec_frame_of(L, gc);
+  const DecFrame F = L.frames[fidx];
+  if (chunk_slot_empty(F, gc)) return;
   if (threadIdx.x == 0) {
     unsigned long long w0, w1;
     do {
@@ -828,18 +827,6 @@ __global__ void __launch_bounds__(kSeT) stream_end_kernel(const DecLaunch L, con
     s_desc[1] = w1 & 0xFFFFFFFFull;
   }
   __syncthreads();
-  uint32_t fidx;
-  if (L.uniform_chunks) {
-    fidx = gc / L.uniform_chunks;
-  } else {
-    uint32_t lo = 0, hi = L.n_frames - 1;
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi + 1) >> 1;
-      if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
-    }
-    fidx = lo;
-  }
-  const DecFrame F = L.frames[fidx];
   const uint32_t n_points = min(kChunkPoints, F.n_points - (gc - F.chunk_begin) * kChunkPoints);
   const uint32_t size = static_cast<uint32_t>(s_desc[1]);
   const uint32_t N = n_points * K;                                   // <= 32768 * 6

@@ -39,12 +39,22 @@ __global__ void count_tiles_kernel(const DecLaunch L) {
     const uint32_t mid = (lo + hi + 1) >> 1;
     if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
   }
+  L.chunk_frame[gc] = lo;
+  if (chunk_slot_empty(L.frames[lo], gc)) {  // no tile
+    L.chunk_tiles[gc] = 0;
+    L.stream_end[gc] = 0xFFFFFFFFu;
+    return;
+  }
   const uint8_t* body = L.frames[lo].payload + L.chunk_offsets[gc];
   const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(body) & 15u);
   const uint32_t size = L.chunk_sizes[gc];
-  L.chunk_tiles[gc] = size ? (size + mis + kTB - 1) / kTB : 0;
-  L.chunk_frame[gc] = lo;
   L.stream_end[gc] = 0xFFFFFFFFu;  // set by the tile that decodes the chunk's last regular value
+  if (L.chunk_bytes_max && size > L.chunk_bytes_max) {  // past the bound the grid was sized from: no tile, the frame fails
+    L.chunk_tiles[gc] = 0;
+    report_frame_error(L, lo, DEV_ERR_CHUNK_SIZE);
+    return;
+  }
+  L.chunk_tiles[gc] = size ? (size + mis + kTB - 1) / kTB : 0;
   const uint32_t chunk = gc - L.frames[lo].chunk_begin;
   const uint32_t n_points = min(kChunkPoints, L.frames[lo].n_points - chunk * kChunkPoints);
   if (size == 0 && n_points * L.plan->values_per_point > 0) report_frame_error(L, lo, DEV_ERR_TRUNCATED);
@@ -803,32 +813,28 @@ __global__ void __launch_bounds__(kDT, kSeqMinBlocks) decode_chunks_seq_kernel(c
       if (i < L.n_chunks_total) {
         // equal frames: claim chunk-index-major (all chunk 0s first), so early claims never wait long for the walk
         if (L.uniform_chunks && !L.redo_mode) gc_ = (i % L.n_frames) * L.uniform_chunks + i / L.n_frames;
-        unsigned long long w0, w1;
-        do {
-          w0 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_);
-          w1 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_ + 1);
-        } while (static_cast<uint32_t>(w0 >> 40) != L.desc_tag || static_cast<uint32_t>(w1 >> 40) != L.desc_tag);
-        s_desc[0] = w0 & 0xFFFFFFFFFFull;
-        s_desc[1] = w1 & 0xFFFFFFFFull;
-        L.stream_end[gc_] = 0xFFFFFFFFu;  // set by the tile that decodes the chunk's last regular value
+        if (!L.empty_slots || !chunk_slot_empty(L.frames[dec_frame_of(L, gc_)], gc_)) {  // nobody publishes an empty slot
+          unsigned long long w0, w1;
+          do {
+            w0 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_);
+            w1 = ld_relaxed_u64(L.chunk_desc + 2ull * gc_ + 1);
+          } while (static_cast<uint32_t>(w0 >> 40) != L.desc_tag || static_cast<uint32_t>(w1 >> 40) != L.desc_tag);
+          s_desc[0] = w0 & 0xFFFFFFFFFFull;
+          s_desc[1] = w1 & 0xFFFFFFFFull;
+          L.stream_end[gc_] = 0xFFFFFFFFu;  // set by the tile that decodes the chunk's last regular value
+        }
       }
       s_chunk = gc_;
     }
     __syncthreads();
     const uint32_t gc = s_chunk;
     if (gc >= L.n_chunks_total) return;
-    uint32_t fidx;
-    if (L.uniform_chunks) {
-      fidx = gc / L.uniform_chunks;
-    } else {
-      uint32_t lo = 0, hi = L.n_frames - 1;
-      while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
-      }
-      fidx = lo;
-    }
+    const uint32_t fidx = dec_frame_of(L, gc);
     const DecFrame F = L.frames[fidx];
+    if (chunk_slot_empty(F, gc)) {
+      __syncthreads();  // everybody has read s_chunk before thread 0 may claim the next chunk
+      continue;
+    }
     const uint32_t chunk = gc - F.chunk_begin;
     const uint32_t n_points = min(kChunkPoints, F.n_points - chunk * kChunkPoints);
     const uint32_t V = n_points * K;

@@ -83,6 +83,8 @@ struct DecLaunch {
   uint32_t sections_only;      // decode_chunks_kernel: the regular stream was decoded elsewhere, start at stream_end[]
   uint32_t tile_capacity;      // records allocated (== tile_grid)
   uint32_t tile_grid;          // host upper bound on the number of tiles
+  uint32_t chunk_bytes_max;    // > 0: tile_grid was sized from a prepared shape whose chunk bodies hold at most this many
+                               // bytes; count_tiles_kernel fails a larger chunk's frame instead of tiling it
   uint32_t epoch;
   // Side mode (V5 sections decoded AHEAD of the regular stream, large batches): stream_end_kernel finds where every chunk's
   // regular stream ends, the section reader writes its values into compact arrays -- section s of global chunk gc at
@@ -93,6 +95,8 @@ struct DecLaunch {
   uint32_t side_mode;          // decode_chunks_kernel, sections_only: 1 = store into the side arrays; any anomaly marks the
                                // chunk (stream_end = 0xFFFFFFFF) for the careful kernels instead of raising the error word
   uint32_t* frame_err;         // nullptr, or one word per frame (zeroed per launch) that takes that frame's errors
+  uint32_t empty_slots;        // 1: some chunk slots are empty (chunk_slot_empty); the chunk-sequential readers check
+                               // a claimed slot before they wait for its descriptor
 };
 
 // Error word of frame f: its own word when the launch has per-frame words, else the launch word (so launches without
@@ -102,6 +106,24 @@ template <class Launch>
 __device__ __forceinline__ uint32_t* frame_err_word(const Launch& L, uint32_t f) { return L.frame_err ? L.frame_err + f : L.err; }
 template <class Launch>
 __device__ __forceinline__ void report_frame_error(const Launch& L, uint32_t f, uint32_t code) { atomicCAS(frame_err_word(L, f), 0u, code); }
+
+// Whether global chunk gc, which lies in frame F's range, is not one of F's chunks. cldn_b200_decode_blobs_async gives every
+// frame the same number of chunk slots (those of the prepared maximum of points), so the slots past a frame's own chunks --
+// all of them for a frame refused before the decode -- are empty, and a kernel leaves an empty slot at once. Every other
+// launch packs the frames' chunks back to back and has no empty slot. (DecFrame and Lz4Frame)
+template <class Frame>
+__device__ __forceinline__ bool chunk_slot_empty(const Frame& F, uint32_t gc) { return gc - F.chunk_begin >= F.n_chunks; }
+
+// Frame of global chunk gc: gc / uniform_chunks, else the last frame that begins at or before gc.
+__device__ __forceinline__ uint32_t dec_frame_of(const DecLaunch& L, uint32_t gc) {
+  if (L.uniform_chunks) return gc / L.uniform_chunks;
+  uint32_t lo = 0, hi = L.n_frames - 1;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi + 1) >> 1;
+    if (L.frames[mid].chunk_begin <= gc) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
 
 int launch_decode(const Plan& host_plan, const DecLaunch& L, cudaStream_t stream);
 int launch_decode_tiles(const Plan& host_plan, const DecLaunch& L, cudaStream_t stream);
@@ -210,6 +232,42 @@ int launch_gather_prefixes(const uint64_t* tab, uint32_t n, uint8_t* dst, cudaSt
 // `slots` (2n words, cldn_b200_encode_mixed_blobs): sizes[slots[n + f]] = from[slots[f]] + that length instead.
 int launch_place_headers(const uint64_t* tab, uint32_t n, uint64_t* sizes, cudaStream_t stream, const uint64_t* from = nullptr,
                          const uint32_t* slots = nullptr);
+
+// ---- complete device blobs of one prepared layout, without the host (cldn_b200_decode_blobs_async; cldn_blobs_async.cu) ---
+struct BlobDesc {  // cldn_blob_desc_t
+  const uint8_t* blob;
+  uint64_t blob_bytes;
+  uint8_t* out;
+  uint64_t capacity;
+};
+struct AsyncLaunch {
+  const BlobDesc* desc;       // device, n_frames
+  uint32_t n_frames;
+  uint32_t n_tables;          // frames of the prepared shape (>= n_frames): the tables of frames n_frames.. are written empty
+  const uint8_t* tmpl;        // the layout's header with width and height cut out: part 0 | part 1 | part 2 ('\0' included)
+  uint32_t tmpl_len[3];
+  uint64_t max_points;
+  uint32_t point_step;
+  uint32_t slots;             // chunk slots per frame (frame f: f * slots ..)
+  uint32_t compression;       // CLDN_COMP_*
+  DecFrame* frames;           // stage 1
+  Lz4Frame* lz_frames;        // stage 2 (LZ4 / ZSTD)
+  uint8_t* s1;                // stage-1 payloads after stage 2: frame f at s1 + f * s1_stride
+  uint64_t s1_stride;
+  const uint64_t* s1_sizes;   // stage 2: bytes of every frame's stage-1 payload (Lz4Launch::sizes)
+  const uint32_t* chunk_sizes;  // stage 2: bytes every chunk decompressed to (Lz4Launch::chunk_sizes)
+  uint64_t chunk_a, chunk_b;  // stage-1 worst case of a chunk of p > 0 points: chunk_a + chunk_b * p bytes
+  uint32_t* frame_err;        // one word per frame, zeroed before the launches
+  uint32_t* err;              // the launches' word (errors no frame claimed)
+  int32_t* status;            // device, n_frames
+  uint64_t* decoded;          // device, n_frames, optional
+};
+// Header check and frame tables; status[f] = CLDN_OK or the header / size refusal.
+int launch_blobs_async_headers(const AsyncLaunch& A, cudaStream_t stream);
+// After stage 2: a frame's stage-1 payload size goes into its DecFrame, a frame stage 2 failed leaves stage 1 out.
+int launch_blobs_async_link(const AsyncLaunch& A, cudaStream_t stream);
+// status[f] / decoded[f] from the frame's error word.
+int launch_blobs_async_status(const AsyncLaunch& A, cudaStream_t stream);
 
 uint64_t kernel_launch_count();
 void count_launch(int n = 1);  // process-wide, atomic: handles on other threads count into the same total

@@ -229,6 +229,7 @@ __global__ void __launch_bounds__(kLzThreads) lz4_decompress_chunks_kernel(const
   if (gc >= L.n_chunks_total) return;
   const uint32_t f = L.chunk_frame[gc];
   const Lz4Frame F = L.frames[f];
+  if (chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   uint64_t body = 0;
   const uint32_t n = lz_find_chunk(F.packed_in, F.packed_in_bytes, c, &body);

@@ -772,6 +772,7 @@ __global__ void __launch_bounds__(kZsThreads) zstd_decompress_chunks_kernel(cons
   for (uint32_t gc = w; gc < L.n_chunks_total; gc += gridDim.x * kZsWarps) {
     const uint32_t f = L.chunk_frame[gc];
     const Lz4Frame F = L.frames[f];
+    if (chunk_slot_empty(F, gc)) continue;
     const uint32_t c = gc - F.chunk_begin;
     uint64_t body = 0;
     const uint32_t n = lz_find_chunk(F.packed_in, F.packed_in_bytes, c, &body);

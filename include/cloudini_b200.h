@@ -276,6 +276,50 @@ int cldn_b200_decode_batch(cldn_decoder_t* dec, const cldn_info_t* info, size_t 
 int cldn_b200_decode_blobs(cldn_decoder_t* dec, size_t n_frames, const void* const* blobs, const size_t* blob_bytes,
                            void* const* outs, const size_t* out_capacities, int mem, int32_t* status,
                            size_t* decoded_bytes);
+/* Device-resident blobs of ONE known layout and any point counts, decoded without the host: for GPU consumers whose blobs
+ * are already in device memory (a training or replay loop over clouds kept compressed in HBM, blobs received with NCCL
+ * or written by cldn_b200_encode_blobs), and for callers that capture the decode in a CUDA graph.
+ *
+ * cldn_b200_decoder_prepare_blobs: once per layout and shape, outside any capture. `layout` is the EncodingInfo of the
+ * blobs (width / height ignored; wire version 3..5; compression NONE, LZ4 or ZSTD). Builds and uploads the plan and the
+ * layout's header, and allocates every device buffer a call of up to `max_frames` frames of up to `max_points_per_frame`
+ * points each needs. Waits for the handle's stream, and for the whole device where it allocates zero-filled scratch (as
+ * the buffer growth of the handle's other calls does). The prepared state is separate from the handle's other calls:
+ * cldn_b200_decode, _decode_batch and _decode_blobs keep working between prepare and async calls and do not invalidate
+ * it. A new prepare replaces it, and graphs captured before it are then invalid.
+ *
+ * cldn_b200_decode_blobs_async: enqueues on the handle's stream and returns. No host synchronisation, allocation,
+ * pageable copy or host->device copy: everything that depends on the frames is read by the kernels, so the call can be
+ * captured in a CUDA graph (on the stream the decoder was created with) and replayed after new blobs and descriptors
+ * were written into the same device buffers. `d_frames`: DEVICE array of n_frames cldn_blob_desc_t (all device
+ * pointers). d_status (int32 per frame) and d_decoded_bytes (uint64 per frame, optional: width * height * point_step,
+ * 0 for a failed frame) are DEVICE arrays, written on the handle's stream. The launches do not depend on n_frames or on
+ * the point counts. The call itself returns CLDN_ERR_INVALID_ARGUMENT without a prepared layout or with
+ * n_frames > max_frames, before anything is enqueued.
+ * d_status[f]:
+ *   CLDN_OK                   the frame holds exactly what cldn_b200_decode_blobs writes for it (padding untouched);
+ *   CLDN_ERR_BAD_HEADER       the blob does not start with the prepared layout's canonical header, i.e. the bytes
+ *                             cldn_b200_encode_header writes for that layout with some width and height, spelled as
+ *                             EncodingInfoToYAML spells them (a valid header of another layout included: use
+ *                             cldn_b200_decode_blobs for those);
+ *   CLDN_ERR_UNSUPPORTED      the header states more than max_points_per_frame points;
+ *   CLDN_ERR_BUFFER_TOO_SMALL width * height * point_step > capacity;
+ *   CLDN_ERR_CORRUPT_DATA     damaged chunks or stage-2 frames, where cldn_b200_decode_blobs gives that status (and a
+ *                             chunk larger than the layout's worst case, which no encoder writes).
+ * A failed frame's output bytes are unspecified; no byte outside any frame's [0, capacity) is written. There are no
+ * messages: after synchronising, decode a failed frame with cldn_b200_decode_blobs for the reference's message.
+ * The kernels are those cldn_b200_decode_blobs picks for the layout, routed by the prepared shape (every frame owns the
+ * chunks of max_points_per_frame points). */
+typedef struct cldn_blob_desc_t {
+  const void* blob;
+  uint64_t blob_bytes;
+  void* out;
+  uint64_t capacity;
+} cldn_blob_desc_t;
+int cldn_b200_decoder_prepare_blobs(cldn_decoder_t* dec, const cldn_info_t* layout, size_t max_frames,
+                                    uint64_t max_points_per_frame);
+int cldn_b200_decode_blobs_async(cldn_decoder_t* dec, size_t n_frames, const void* d_frames, int32_t* d_status,
+                                 uint64_t* d_decoded_bytes);
 /* Message of frame f of this handle's last cldn_b200_decode_blobs ("" when it decoded). */
 const char* cldn_b200_decoder_frame_error(const cldn_decoder_t* dec, size_t f);
 /* EncodingInfo read from the header of frame f of this handle's last cldn_b200_decode_blobs (zeroed when the header
