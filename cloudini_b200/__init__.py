@@ -21,7 +21,7 @@ __all__ = [
     "FieldType", "EncodingOptions", "CompressionOption", "PointField", "EncodingInfo", "EncodingInfoToYAML",
     "EncodingInfoFromYAML", "EncodeHeader", "DecodeHeader", "MaxCompressedSize", "PointcloudEncoder", "MixedEncoder",
     "PointcloudDecoder", "SizeOf", "lib", "library_path", "kernel_launch_count", "kDecodeButSkipStore", "blob_descs",
-    "pack_blob_descs",
+    "pack_blob_descs", "cloud_descs", "pack_cloud_descs",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -144,6 +144,8 @@ def lib():
     L.cldn_b200_encoder_sizes_device.restype = vp
     L.cldn_b200_encoder_sync.argtypes = [vp]
     L.cldn_b200_encoder_set_stage2_on_device.argtypes = [vp, C.c_int]
+    L.cldn_b200_encoder_prepare_blobs.argtypes = [vp, sz, C.c_uint64]
+    L.cldn_b200_encode_blobs_async.argtypes = [vp, sz, vp, vp, vp]
     L.cldn_b200_mixed_encoder_create.argtypes = [C.c_int, vp, C.POINTER(vp)]
     L.cldn_b200_mixed_encoder_destroy.argtypes = [vp]
     L.cldn_b200_mixed_encoder_destroy.restype = None
@@ -452,6 +454,17 @@ class PointcloudEncoder:
                                             MEM_DEVICE_POINTS))
         return [outs[f][:written[f]].tobytes() for f in range(n)]
 
+    def prepare_blobs(self, max_frames: int, max_points: int):
+        """Prepares encode_blobs_async() for calls of at most `max_frames` clouds of at most `max_points` points each, in
+        this encoder's layout and with its stage-2 setting now. See cldn_b200_encoder_prepare_blobs."""
+        _check(lib().cldn_b200_encoder_prepare_blobs(self._h, max_frames, max_points))
+
+    def encode_blobs_async(self, frames_ptr: int, n: int, status_ptr: int, written_ptr: int = 0):
+        """Enqueues the encode of n device clouds into complete device blobs on the encoder's stream and returns (graph
+        capturable). frames_ptr: device address of n descriptors (pack_cloud_descs); status_ptr: device int32[n];
+        written_ptr: device uint64[n] of blob sizes, or 0. Statuses: see cldn_b200_encode_blobs_async."""
+        _check(lib().cldn_b200_encode_blobs_async(self._h, n, frames_ptr or None, status_ptr or None, written_ptr or None))
+
     def sizes_device_ptr(self) -> int:
         return int(lib().cldn_b200_encoder_sizes_device(self._h) or 0)
 
@@ -565,6 +578,30 @@ def pack_blob_descs(descs: Sequence, out=None):
     Returns the tensor; its data_ptr() is decode_blobs_async()'s frames_ptr."""
     import torch
     host = torch.from_numpy(blob_descs(descs).view("uint8").reshape(-1))
+    if out is None:
+        return host.cuda()
+    out.view(torch.uint8).reshape(-1)[:host.numel()].copy_(host)
+    return out
+
+
+def cloud_descs(descs: Sequence):
+    """numpy uint64 array [n, 5] of cldn_cloud_desc_t: one (cloud_ptr, cloud_bytes, out_ptr, capacity[, width, height])
+    per frame, device addresses and sizes as encode_blobs_async() reads them; width = height = 0 (or left out) for
+    (points, 1)."""
+    import numpy as np
+    a = np.zeros((len(descs), 5), dtype=np.uint64)
+    for f, d in enumerate(descs):
+        cloud, nbytes, out, cap = (int(v) for v in d[:4])
+        w, h = (int(d[4]), int(d[5])) if len(d) > 4 else (0, 0)
+        a[f] = [cloud, nbytes, out, cap, w | (h << 32)]
+    return a
+
+
+def pack_cloud_descs(descs: Sequence, out=None):
+    """The descriptors of cloud_descs() in device memory, as pack_blob_descs() does for blob_descs() (40 bytes per
+    frame). Returns the tensor; its data_ptr() is encode_blobs_async()'s frames_ptr."""
+    import torch
+    host = torch.from_numpy(cloud_descs(descs).view("uint8").reshape(-1))
     if out is None:
         return host.cuda()
     out.view(torch.uint8).reshape(-1)[:host.numel()].copy_(host)

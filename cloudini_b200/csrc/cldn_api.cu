@@ -329,8 +329,12 @@ struct EncScratch {
   PinRing<uint8_t> h_blob_headers;
 };
 
+struct AsyncEncode;  // cldn_b200_encoder_prepare_blobs
+struct AsyncEncodeDeleter { void operator()(AsyncEncode* a) const; };
+
 struct cldn_encoder : EncLayout, EncScratch {
   bool pooled = false;  // a handle of the per-thread pool (encoder_mark_pooled): keeps the libraries' bytes
+  std::unique_ptr<AsyncEncode, AsyncEncodeDeleter> async;  // the prepared shape of cldn_b200_encode_blobs_async
 };
 
 // cldn_b200_encoder_create's refusals, in its order, and the host part of the layout of `info`.
@@ -366,6 +370,22 @@ static int upload_layout(EncLayout& l) {
 
 // LZ4_COMPRESSBOUND (lz4.h): worst case of a block for n input bytes
 static size_t lz4_bound(size_t n) { return n + n / 255 + 16; }
+
+// The header of a layout with width = height = 0, cut around the two numbers: tmpl = part 0 | part 1 | part 2 with
+// len[k] bytes each, so that the header of dims (w, h) is part 0, "%u" of w, part 1, "%u" of h, part 2. The headers the
+// prepared async calls write (encode) and accept (decode) are built from it on the device.
+static int header_template(const std::vector<uint8_t>& hdr, std::vector<uint8_t>* tmpl, uint32_t len[3]) {
+  const std::string text(reinterpret_cast<const char*>(hdr.data()), hdr.size());
+  const size_t w_at = text.find("\nwidth: 0\nheight: 0\n");
+  if (w_at == std::string::npos) { set_error("the layout's header has no width / height lines"); return CLDN_ERR_INTERNAL; }
+  len[0] = static_cast<uint32_t>(w_at + 8);
+  len[1] = 9;
+  len[2] = static_cast<uint32_t>(hdr.size() - (w_at + 19));
+  tmpl->assign(hdr.begin(), hdr.begin() + len[0]);
+  tmpl->insert(tmpl->end(), hdr.begin() + len[0] + 1, hdr.begin() + len[0] + 1 + len[1]);
+  tmpl->insert(tmpl->end(), hdr.begin() + w_at + 19, hdr.end());
+  return CLDN_OK;
+}
 
 namespace cldn {
 void encoder_mark_pooled(cldn_encoder_t* enc) { enc->pooled = true; }
@@ -617,6 +637,44 @@ static int stage_layout(DevBuf<uint8_t>& buf, size_t n, const size_t* bytes, std
   return CLDN_OK;
 }
 
+// Stage 1 from launch structs: the V5 sections (S, when the plan has them), the Gorilla pre-pass, the regular stream
+// and the placement of the sections. cldn_b200_encode_batch and the prepared async call enqueue this same sequence.
+static int launch_encode_stage1(const Plan& plan, const EncLaunch& L, const SecLaunch* S, cudaStream_t stream) {
+  if (S && launch_encode_sections(plan, *S, stream) < 0) { set_error("section kernel launch failed"); return CLDN_ERR_CUDA; }
+  if (launch_gorilla_prepass(plan, L, stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
+  if (launch_encode_regular(plan, L, stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
+  if (S && launch_place_sections(plan, *S, L.status, L.epoch, L.tile_points, stream) < 0) {
+    set_error("section placement launch failed");
+    return CLDN_ERR_CUDA;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return CLDN_OK;
+}
+
+// Stage 2 from its launch struct: the LZ4 or ZSTD chunk coder, then the pack into the blobs.
+static int launch_encode_stage2(bool zstd, const Lz4Launch& Z, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream) {
+  if (zstd) {
+    if (launch_zstd_compress(Z, header, header_bytes, stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
+  } else if (launch_lz4_compress(Z, header, header_bytes, stream) < 0) {
+    set_error("LZ4 kernel launch failed");
+    return CLDN_ERR_CUDA;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return CLDN_OK;
+}
+
+// Bytes of one (chunk, section) slot of the V5 section scratch: the worst case of any mode is DeltaRle with one run per
+// value, 5 + n * (max varint of the field + 1) bytes, plus the 16 bytes the vector copy of place_sections_kernel may read
+// past the end.
+static uint32_t section_stride(const Plan& plan) {
+  uint32_t per_value = 0;
+  for (uint32_t k = 0; k < plan.n_sections; ++k) {
+    const uint32_t bpv = plan.sections[k].bpv;
+    per_value = std::max<uint32_t>(per_value, (bpv == 2 ? 3u : bpv == 4 ? 5u : 10u) + 1u);
+  }
+  return 32 + kChunkPoints * per_value;
+}
+
 // Stage 1 of frames that passed check_encode_frame, or of staging their caller sized: fills their EncFrames and enqueues
 // the kernels. Inputs and outputs are device pointers; the kernels check every store against out_capacities.
 static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
@@ -667,7 +725,7 @@ static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frame
     CUDA_TRY(cudaMemsetAsync(s.d_status.p, 0, s.d_status.cap * sizeof(uint64_t), s.stream));
     s.epoch = 1;
   }
-  EncLaunch L;
+  EncLaunch L{};
   L.frames = s.d_frames.p;
   L.n_frames = static_cast<uint32_t>(n_frames);
   L.n_tiles_total = static_cast<uint32_t>(tiles);
@@ -688,16 +746,11 @@ static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frame
     if (uniform) L.uniform_tiles = hf[0].n_tiles;
   }
 
+  SecLaunch S{};
   if (l.plan.n_sections > 0) {
     // V5: adaptive integer sections are produced first (they determine where every later chunk starts).
     const uint32_t ns = l.plan.n_sections;
-    // worst case of any mode is DeltaRle with one run per value: 5 + n * (max varint of the field + 1) bytes
-    uint32_t per_value = 0;
-    for (uint32_t k = 0; k < ns; ++k) {
-      const uint32_t bpv = l.plan.sections[k].bpv;
-      per_value = std::max<uint32_t>(per_value, (bpv == 2 ? 3u : bpv == 4 ? 5u : 10u) + 1u);
-    }
-    const uint32_t stride = 32 + kChunkPoints * per_value;   // 5 header bytes + 16 bytes the vector copy of place_sections_kernel may read past the end
+    const uint32_t stride = section_stride(l.plan);
     if (int rc = s.d_modes.reserve(n_frames * ns)) return rc;
     if (int rc = s.d_sec_scratch.reserve(static_cast<size_t>(chunks) * ns * stride)) return rc;
     if (int rc = s.d_sec_sizes.reserve(static_cast<size_t>(chunks) * ns + 1)) return rc;
@@ -717,9 +770,6 @@ static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frame
     }
     CUDA_TRY(cudaMemcpyAsync(s.d_chunk_frame.p, hcf, (chunks + n_frames) * sizeof(uint32_t), cudaMemcpyHostToDevice, s.stream));
     if (int rc = s.h_chunk_frame.commit(hcf_slot, s.stream)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(s.d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, s.stream));
-    if (int rc = s.h_frames.commit(hf_slot, s.stream)) return rc;
-    SecLaunch S{};
     S.frames = s.d_frames.p;
     S.n_frames = static_cast<uint32_t>(n_frames);
     S.n_chunks_total = static_cast<uint32_t>(chunks);
@@ -734,18 +784,10 @@ static int encode_batch_device(const EncLayout& l, EncScratch& s, size_t n_frame
     S.hash_scratch = s.d_hash.p;
     S.err = s.d_err.p;
     S.header_bytes = static_cast<uint32_t>(hdr);
-    if (launch_encode_sections(l.plan, S, s.stream) < 0) { set_error("section kernel launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_gorilla_prepass(l.plan, L, s.stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_encode_regular(l.plan, L, s.stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_place_sections(l.plan, S, s.d_status.p, s.epoch, T, s.stream) < 0) { set_error("section placement launch failed"); return CLDN_ERR_CUDA; }
-  } else {
-    CUDA_TRY(cudaMemcpyAsync(s.d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, s.stream));
-    if (int rc = s.h_frames.commit(hf_slot, s.stream)) return rc;
-    if (launch_gorilla_prepass(l.plan, L, s.stream) < 0) { set_error("gorilla pre-pass launch failed"); return CLDN_ERR_CUDA; }
-    if (launch_encode_regular(l.plan, L, s.stream) < 0) { set_error("encode kernel launch failed"); return CLDN_ERR_CUDA; }
   }
-  CUDA_TRY(cudaGetLastError());
-  return CLDN_OK;
+  CUDA_TRY(cudaMemcpyAsync(s.d_frames.p, hf, n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice, s.stream));
+  if (int rc = s.h_frames.commit(hf_slot, s.stream)) return rc;
+  return launch_encode_stage1(l.plan, L, l.plan.n_sections > 0 ? &S : nullptr, s.stream);
 }
 
 // Stage 1 into an internal arena, then stage 2 on the device: one LZ4 block per chunk (cldn_lz4.cu) or one ZSTD frame
@@ -820,13 +862,8 @@ static int encode_batch_device_stage2(const EncLayout& l, EncScratch& s, size_t 
   if (zstd) {
     Z.block_begin = s.d_lz_chunk_frame.p + chunks;
     Z.n_blocks_total = static_cast<uint32_t>(pieces);
-    if (launch_zstd_compress(Z, l.d_header.p, static_cast<uint32_t>(hdr), s.stream) < 0) { set_error("ZSTD kernel launch failed"); return CLDN_ERR_CUDA; }
-  } else if (launch_lz4_compress(Z, l.d_header.p, static_cast<uint32_t>(hdr), s.stream) < 0) {
-    set_error("LZ4 kernel launch failed");
-    return CLDN_ERR_CUDA;
   }
-  CUDA_TRY(cudaGetLastError());
-  return CLDN_OK;
+  return launch_encode_stage2(zstd, Z, l.d_header.p, static_cast<uint32_t>(hdr), s.stream);
 }
 
 // Host blobs (CLDN_MEM_HOST, CLDN_MEM_DEVICE_POINTS) through device staging bounded by caps[f]: the clouds go up on the
@@ -1009,6 +1046,216 @@ static int encode_blobs_impl(cldn_encoder_t* e, size_t n_frames, const void* con
   return read_written(*e, n_frames, written_host);
 }
 
+// ---- device clouds of the encoder's layout, without the host (cldn_b200_encode_blobs_async) --------------------------
+// Everything the calls of one prepared shape read: uploaded and allocated once by cldn_b200_encoder_prepare_blobs, apart
+// from the handle's other scratch, so that a call allocates, copies from the host and synchronises nothing, and a CUDA
+// graph that captured one stays valid until the next prepare. Every frame owns the tile and chunk slots of max_points;
+// the frame kernel fills a frame's own and the encode kernels leave the rest (EncLaunch / SecLaunch / Lz4Launch
+// ::empty_slots). Tile status words and error words are cleared inside every call, so a replayed graph starts clean.
+struct AsyncEncode {
+  size_t max_frames = 0;
+  bool stage2 = false, zstd = false;
+  DevBuf<uint8_t> d_tmpl;
+  DevBuf<EncFrame> d_frames;
+  DevBuf<Lz4Frame> d_lz_frames;
+  DevBuf<uint64_t> d_sizes, d_status, d_hash;
+  DevBuf<uint32_t> d_ticket, d_hdr_len, d_frame_err, d_err;
+  DevBuf<uint8_t> d_gorilla, d_modes, d_sec_scratch, d_s1, d_lz_scratch;
+  DevBuf<uint32_t> d_sec_sizes, d_sec_excl, d_chunk_frame, d_lz_chunk_frame, d_lz_chunk_sizes;
+  EncAsyncLaunch A{};  // all but the call's arrays
+  EncLaunch L{};
+  SecLaunch S{};
+  Lz4Launch Z{};
+};
+void AsyncEncodeDeleter::operator()(AsyncEncode* a) const { delete a; }
+
+static int encoder_prepare_blobs_impl(cldn_encoder* e, size_t max_frames, uint64_t max_points) {
+  if (!e) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_frames == 0 || max_frames > 0x7FFFFFFFull) { set_error("max_frames must be 1 .. 2^31 - 1"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_points > 0xFFFFFFFFull) { set_error("max_points_per_frame must be below 2^32"); return CLDN_ERR_UNSUPPORTED; }
+  EncodeRoute route;
+  if (int rc = choose_encode_route(*e, *e, CLDN_MEM_DEVICE, &route)) return rc;
+  const Plan& plan = e->plan;
+  const uint32_t T = e->tile_points;
+  const uint64_t slots = (max_points + kChunkPoints - 1) / kChunkPoints, tiles_per_frame = (max_points + T - 1) / T;
+  const uint64_t chunks = max_frames * slots, tiles = max_frames * tiles_per_frame;
+  if (chunks > 0x7FFFFFFFull || tiles > 0x7FFFFFFFull) { set_error("max_frames * tiles or chunks per frame must be below 2^31"); return CLDN_ERR_UNSUPPORTED; }
+  // MaxCompressedSize terms: a chunk of p points takes 4 + bound(p * per_point + chunk_extra) bytes
+  bool ok1, ok2, ok3, ok4;
+  const size_t m1 = max_compressed_size(e->info, 1, false, &ok1), m2 = max_compressed_size(e->info, 2, false, &ok2);
+  const size_t full = max_compressed_size(e->blob_info, kChunkPoints, false, &ok3), full_s1 = max_compressed_size(e->info, kChunkPoints, false, &ok4);
+  if (!ok1 || !ok2 || !ok3 || !ok4) return CLDN_ERR_INVALID_ARGUMENT;
+  CUDA_TRY(cudaSetDevice(e->device));
+  CUDA_TRY(cudaStreamSynchronize(e->stream));  // kernels of an earlier prepared state may still read it
+  e->async.reset();
+  std::unique_ptr<AsyncEncode, AsyncEncodeDeleter> a(new AsyncEncode());
+  a->max_frames = max_frames;
+  a->stage2 = route == kEncDeviceStage2;
+  a->zstd = a->stage2 && e->stage2 == CLDN_COMP_ZSTD;
+  cldn_info_t zero = e->blob_info;
+  zero.width = zero.height = 0;
+  std::vector<uint8_t> tmpl;
+  EncAsyncLaunch& A = a->A;
+  if (int rc = header_template(make_header(zero), &tmpl, A.tmpl_len)) return rc;
+  std::vector<uint32_t> tables;  // host copies of the shape's tables, alive until the uploads below have completed
+  std::vector<uint32_t> lz_tables;
+
+  if (int rc = a->d_tmpl.reserve(tmpl.size())) return rc;
+  CUDA_TRY(cudaMemcpyAsync(a->d_tmpl.p, tmpl.data(), tmpl.size(), cudaMemcpyHostToDevice, e->stream));
+  if (int rc = a->d_frames.reserve(max_frames)) return rc;
+  if (int rc = a->d_sizes.reserve(max_frames)) return rc;
+  if (int rc = a->d_hdr_len.reserve(max_frames)) return rc;
+  if (int rc = a->d_frame_err.reserve(max_frames)) return rc;
+  if (int rc = a->d_err.reserve(1, true)) return rc;
+  if (int rc = a->d_status.reserve(tiles + 1)) return rc;
+  if (int rc = a->d_ticket.reserve(1)) return rc;
+  A.tmpl = a->d_tmpl.p;
+  A.point_step = e->info.point_step;
+  A.max_points = max_points;
+  A.per_point = m2 - m1;
+  A.chunk_extra = static_cast<uint32_t>(m1 - 4 - (m2 - m1));
+  A.compression = e->stage2;
+  A.full_chunk = full;
+  A.full_chunk_s1 = full_s1;
+  A.tile_points = T;
+  A.tiles_per_frame = static_cast<uint32_t>(tiles_per_frame);
+  A.slots = static_cast<uint32_t>(slots);
+  A.frames = a->d_frames.p;
+  A.sizes = a->d_sizes.p;
+  A.hdr_len = a->d_hdr_len.p;
+  A.frame_err = a->d_frame_err.p;
+  A.err = a->d_err.p;
+  A.n_tables = static_cast<uint32_t>(max_frames);
+
+  EncLaunch& L = a->L;
+  L.frames = a->d_frames.p;
+  L.n_frames = static_cast<uint32_t>(max_frames);
+  L.n_tiles_total = static_cast<uint32_t>(tiles);
+  L.plan = e->d_plan.p;
+  L.header = nullptr;  // the frame kernel writes the headers
+  L.header_bytes = 0;
+  L.status = a->d_status.p;
+  L.epoch = 1;         // the words are cleared in every call
+  L.sizes = a->d_sizes.p;
+  L.err = a->d_err.p;
+  L.tile_points = T;
+  L.flags = kEncAlignPerFrame;
+  L.uniform_tiles = static_cast<uint32_t>(tiles_per_frame);
+  L.tile_ticket = a->d_ticket.p;
+  L.frame_err = a->d_frame_err.p;
+  L.empty_slots = 1;
+  if (plan.n_gorilla > 0) {
+    A.side_stride = max_points * 12 * plan.n_gorilla;
+    if (int rc = a->d_gorilla.reserve(max_frames * A.side_stride + 16)) return rc;
+    A.side = a->d_gorilla.p;
+  }
+  if (plan.n_sections > 0) {
+    // chunk slot gc belongs to frame gc / slots; chunk_first[f] = f * slots; frame f's sec_excl at f * (slots + 1)
+    const uint32_t ns = plan.n_sections, stride = section_stride(plan);
+    if (int rc = a->d_modes.reserve(max_frames * ns)) return rc;
+    if (int rc = a->d_sec_scratch.reserve(chunks * ns * stride)) return rc;
+    if (int rc = a->d_sec_sizes.reserve(chunks * ns + 1)) return rc;
+    if (int rc = a->d_sec_excl.reserve(chunks + max_frames + 1)) return rc;
+    if (int rc = a->d_chunk_frame.reserve(chunks + max_frames + 1)) return rc;
+    if (int rc = a->d_hash.reserve(palette_overflow_scratch_bytes() / 8 + 16)) return rc;
+    tables.resize(chunks + max_frames);
+    for (uint64_t gc = 0; gc < chunks; ++gc) tables[gc] = static_cast<uint32_t>(gc / slots);
+    for (size_t f = 0; f < max_frames; ++f) tables[chunks + f] = static_cast<uint32_t>(f * slots);
+    CUDA_TRY(cudaMemcpyAsync(a->d_chunk_frame.p, tables.data(), tables.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    A.sec_excl = a->d_sec_excl.p;
+    SecLaunch& S = a->S;
+    S.frames = a->d_frames.p;
+    S.n_frames = static_cast<uint32_t>(max_frames);
+    S.n_chunks_total = static_cast<uint32_t>(chunks);
+    S.chunk_frame = a->d_chunk_frame.p;
+    S.chunk_first = a->d_chunk_frame.p + chunks;
+    S.plan = e->d_plan.p;
+    S.modes = a->d_modes.p;
+    S.scratch = a->d_sec_scratch.p;
+    S.sec_stride = stride;
+    S.sec_sizes = a->d_sec_sizes.p;
+    S.sec_excl = a->d_sec_excl.p;
+    S.hash_scratch = a->d_hash.p;
+    S.err = a->d_err.p;
+    S.header_bytes = 0;
+    S.frame_err = a->d_frame_err.p;
+    S.empty_slots = 1;
+  }
+  if (a->stage2) {
+    // stage-1 arenas of max_points (a frame's own stores are bounded by its stage1_arena_bytes), and the slots of
+    // encode_batch_device_stage2 for chunks of min(max_points, kChunkPoints) points
+    const uint64_t s1_stride = (stage1_arena_bytes(*e, max_points) + 255) & ~uint64_t(255);
+    bool ok;
+    const size_t chunk_bound = max_compressed_size(e->info, std::min<uint64_t>(max_points, kChunkPoints), false, &ok) + 64;
+    const size_t zblock = zstd_enc_block_bytes();
+    const uint64_t per_chunk = a->zstd ? std::max<size_t>(1, (chunk_bound + zblock - 1) / zblock) : 1, pieces = chunks * per_chunk;
+    const size_t slot = a->zstd ? zstd_enc_slot_bytes() : (lz4_bound(chunk_bound) + 15) & ~size_t(15);
+    if (pieces > 0x7FFFFFFFull) { set_error("max_frames * ZSTD blocks per frame must be below 2^31"); return CLDN_ERR_UNSUPPORTED; }
+    if (slot > 0xFFFFFFF0ull) { set_error("chunk too large for LZ4"); return CLDN_ERR_UNSUPPORTED; }
+    if (int rc = a->d_s1.reserve(std::max<uint64_t>(max_frames * s1_stride, 256))) return rc;
+    if (int rc = a->d_lz_frames.reserve(max_frames)) return rc;
+    if (int rc = a->d_lz_scratch.reserve(std::max<uint64_t>(pieces, 1) * slot)) return rc;
+    if (int rc = a->d_lz_chunk_sizes.reserve(pieces + 1)) return rc;
+    if (int rc = a->d_lz_chunk_frame.reserve(2 * chunks + 2)) return rc;  // chunk -> frame, then block_begin (ZSTD)
+    lz_tables.resize(2 * chunks + 1);
+    for (uint64_t gc = 0; gc < chunks; ++gc) {
+      lz_tables[gc] = static_cast<uint32_t>(gc / slots);
+      lz_tables[chunks + gc] = static_cast<uint32_t>(gc * per_chunk);
+    }
+    lz_tables[2 * chunks] = static_cast<uint32_t>(pieces);
+    CUDA_TRY(cudaMemcpyAsync(a->d_lz_chunk_frame.p, lz_tables.data(), lz_tables.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    A.lz_frames = a->d_lz_frames.p;
+    A.s1 = a->d_s1.p;
+    A.s1_stride = s1_stride;
+    Lz4Launch& Z = a->Z;
+    Z.frames = a->d_lz_frames.p;
+    Z.n_frames = static_cast<uint32_t>(max_frames);
+    Z.n_chunks_total = static_cast<uint32_t>(chunks);
+    Z.chunk_frame = a->d_lz_chunk_frame.p;
+    Z.scratch = a->d_lz_scratch.p;
+    Z.slot_stride = static_cast<uint32_t>(slot);
+    Z.chunk_sizes = a->d_lz_chunk_sizes.p;
+    Z.sizes = a->d_sizes.p;   // the pack kernel overwrites the stage-1 sizes with the payload sizes
+    Z.err = a->d_err.p;
+    Z.frame_err = a->d_frame_err.p;
+    Z.empty_slots = 1;
+    if (a->zstd) {
+      Z.block_begin = a->d_lz_chunk_frame.p + chunks;
+      Z.n_blocks_total = static_cast<uint32_t>(pieces);
+    }
+  }
+  CUDA_TRY(cudaStreamSynchronize(e->stream));  // the uploads read host objects of this function
+  e->async = std::move(a);
+  return CLDN_OK;
+}
+
+// Enqueues only. The launches and their grids are those of the prepared shape, whatever the frames: two clears, the
+// frame kernel, the stage-1 sequence of encode_batch, stage 2 when compressed, the status kernel.
+static int encode_blobs_async_impl(cldn_encoder* e, size_t n, const void* d_frames, int32_t* d_status, uint64_t* d_written) {
+  if (!e) { set_error("null encoder"); return CLDN_ERR_INVALID_ARGUMENT; }
+  AsyncEncode* a = e->async.get();
+  if (!a) { set_error("no prepared shape: call cldn_b200_encoder_prepare_blobs first"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n > a->max_frames) { set_error("%zu frames: the shape was prepared for at most %zu", n, a->max_frames); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (!d_frames || !d_status) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return CLDN_OK;
+  CUDA_TRY(cudaSetDevice(e->device));
+  EncAsyncLaunch A = a->A;
+  A.desc = static_cast<const CloudDesc*>(d_frames);
+  A.n_frames = static_cast<uint32_t>(n);
+  A.status = d_status;
+  A.written = d_written;
+  CUDA_TRY(cudaMemsetAsync(a->d_frame_err.p, 0, a->max_frames * sizeof(uint32_t), e->stream));
+  CUDA_TRY(cudaMemsetAsync(a->d_status.p, 0, a->L.n_tiles_total * sizeof(uint64_t), e->stream));
+  launch_encode_async_frames(A, e->stream);
+  if (int rc = launch_encode_stage1(e->plan, a->L, e->plan.n_sections > 0 ? &a->S : nullptr, e->stream)) return rc;
+  if (a->stage2) {
+    if (int rc = launch_encode_stage2(a->zstd, a->Z, nullptr, 0, e->stream)) return rc;
+  }
+  launch_encode_async_status(A, e->stream);
+  CUDA_TRY(cudaGetLastError());
+  return CLDN_OK;
+}
+
 extern "C" {
 
 int cldn_b200_encode_batch(cldn_encoder_t* e, size_t n_frames, const void* const* clouds, const size_t* cloud_bytes,
@@ -1028,6 +1275,14 @@ int cldn_b200_encode_blobs(cldn_encoder_t* e, size_t n_frames, const void* const
                            const uint32_t* widths, const uint32_t* heights, void* const* outs, const size_t* out_capacities,
                            size_t* written_host, int mem) {
   return guarded([&] { return encode_blobs_impl(e, n_frames, clouds, cloud_bytes, widths, heights, outs, out_capacities, written_host, mem); });
+}
+
+int cldn_b200_encoder_prepare_blobs(cldn_encoder_t* enc, size_t max_frames, uint64_t max_points_per_frame) {
+  return guarded([&] { return encoder_prepare_blobs_impl(enc, max_frames, max_points_per_frame); });
+}
+
+int cldn_b200_encode_blobs_async(cldn_encoder_t* enc, size_t n_frames, const void* d_frames, int32_t* d_status, uint64_t* d_written) {
+  return guarded([&] { return encode_blobs_async_impl(enc, n_frames, d_frames, d_status, d_written); });
 }
 
 }  // extern "C"
@@ -1981,13 +2236,9 @@ static int prepare_blobs_impl(cldn_decoder* d, const cldn_info_t* layout, size_t
   const std::vector<uint8_t> hdr = make_header(zero);
   size_t used = 0;
   if (int rc = cldn_b200_decode_header(hdr.data(), hdr.size(), &a->info, &used)) return rc;
-  const std::string text(reinterpret_cast<const char*>(hdr.data()), hdr.size());
-  const size_t w_at = text.find("\nwidth: 0\nheight: 0\n");
-  if (w_at == std::string::npos) { set_error("the layout's header has no width / height lines"); return CLDN_ERR_INTERNAL; }
-  const uint32_t len0 = static_cast<uint32_t>(w_at + 8), len1 = 9, len2 = static_cast<uint32_t>(hdr.size() - (w_at + 19));
-  std::vector<uint8_t> tmpl(hdr.begin(), hdr.begin() + len0);
-  tmpl.insert(tmpl.end(), hdr.begin() + len0 + 1, hdr.begin() + len0 + 1 + len1);
-  tmpl.insert(tmpl.end(), hdr.begin() + w_at + 19, hdr.end());
+  std::vector<uint8_t> tmpl;
+  uint32_t tmpl_len[3];
+  if (int rc = header_template(hdr, &tmpl, tmpl_len)) return rc;
   cldn_info_t plain = a->info;
   plain.compression_opt = CLDN_COMP_NONE;
   if (int rc = make_decode_plan(plain, &a->plan)) return rc;
@@ -2023,9 +2274,7 @@ static int prepare_blobs_impl(cldn_decoder* d, const cldn_info_t* layout, size_t
   if (int rc = a->d_err.reserve(1, true)) return rc;
   AsyncLaunch& A = a->A;
   A.tmpl = a->d_tmpl.p;
-  A.tmpl_len[0] = len0;
-  A.tmpl_len[1] = len1;
-  A.tmpl_len[2] = len2;
+  for (int k = 0; k < 3; ++k) A.tmpl_len[k] = tmpl_len[k];
   A.max_points = max_points;
   A.point_step = a->info.point_step;
   A.slots = a->slots;

@@ -127,7 +127,7 @@ __device__ __forceinline__ void finish_tile(const EncLaunch& L, const EncFrame& 
   const uint64_t at = 4ull * (chunk + 1) + excl + sec_before;
   const bool fits = L.header_bytes + at + total <= F.out_cap;  // "Output buffer too small for uncompressed chunk"
   if (fits) copy_stage_to_global(stage, total, payload + at);
-  else if (threadIdx.x == 0) report_error(L.err, DEV_ERR_ENCODE_OUTPUT_SMALL);
+  else if (threadIdx.x == 0) report_frame_error(L, frame_idx, DEV_ERR_ENCODE_OUTPUT_SMALL);
   if (t == 0 && L.header_bytes <= F.out_cap) {
     for (uint32_t i = threadIdx.x; i < L.header_bytes; i += blockDim.x) F.out[i] = L.header[i];
   }
@@ -169,6 +169,7 @@ __global__ void __launch_bounds__(kThreads) encode_generic_kernel(const EncLaunc
   const uint32_t fi = L.uniform_tiles ? blockIdx.x % L.n_frames : find_frame(L.frames, L.n_frames, blockIdx.x);
   const EncFrame F = L.frames[fi];
   const uint32_t t = L.uniform_tiles ? blockIdx.x / L.n_frames : blockIdx.x - F.tile_begin;
+  if (L.empty_slots && t >= F.n_tiles) return;  // an empty tile slot (EncLaunch::empty_slots)
   const uint32_t tile = F.tile_begin + t;  // index of the tile's status word
   const uint32_t T = kThreads * I;
   const uint32_t p0 = t * T + threadIdx.x * I;
@@ -253,8 +254,11 @@ __global__ void __launch_bounds__(kThreads, MINB) encode_floatn_kernel(const Enc
   const uint32_t fi = L.uniform_tiles ? blockIdx.x % L.n_frames : find_frame(L.frames, L.n_frames, blockIdx.x);
   const EncFrame F = L.frames[fi];
   const uint32_t t = L.uniform_tiles ? blockIdx.x / L.n_frames : blockIdx.x - F.tile_begin;
+  if (L.empty_slots && t >= F.n_tiles) return;  // an empty tile slot (EncLaunch::empty_slots)
   const uint32_t tile = F.tile_begin + t;  // index of the tile's status word
   constexpr uint32_t T = kThreads * I;
+  // VEC4 launches whose frames' alignment only the device knows take the 16-byte loads frame by frame
+  const bool vec4 = VEC4 && enc_input_aligned16(L.flags, F.in);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t tile_p0 = t * T;
   const uint32_t warp_p0 = tile_p0 + warp * 32 * I;
@@ -266,7 +270,7 @@ __global__ void __launch_bounds__(kThreads, MINB) encode_floatn_kernel(const Enc
   for (int i = 0; i < I; ++i) {
     const uint32_t p = warp_p0 + 32 * i + lane;
     if (p < F.n_points) {
-      if (VEC4) {
+      if (vec4) {
         const float4 q = __ldcs(reinterpret_cast<const float4*>(F.in) + p);
         v[i][0] = q.x; v[i][1] = q.y; v[i][2] = q.z;
         if (N == 4) v[i][N - 1] = q.w;
@@ -627,7 +631,8 @@ int launch_encode_regular(const Plan& plan, const EncLaunch& L, cudaStream_t str
     const RegOp& op = plan.ops[0];
     const bool packed4 = op.lanes == 4 && plan.point_step == 16 && op.offset[0] == 0 && op.offset[1] == 4 &&
                          op.offset[2] == 8 && op.offset[3] == 12;
-    const bool vec4 = packed4 && (L.flags & kEncInputsAligned16);  // LDG.128 needs 16-byte aligned frame bases
+    // LDG.128 needs 16-byte aligned frame bases (kEncAlignPerFrame: the kernel checks each frame's)
+    const bool vec4 = packed4 && (L.flags & (kEncInputsAligned16 | kEncAlignPerFrame));
     if (L.tile_points != kThreads * 8) return -1;
     if (op.lanes == 4) return launch_floatn<4, 8, 3>(plan, L, vec4, stream);
     return launch_floatn<3, 8, 3>(plan, L, false, stream);

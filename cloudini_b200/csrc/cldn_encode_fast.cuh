@@ -149,13 +149,17 @@ __device__ __forceinline__ void tile_coords(const EncLaunch& L, uint32_t i, uint
   }
 }
 
+// PREPARED: the launch of a prepared shape (EncLaunch::empty_slots, kEncAlignPerFrame), whose empty tile slots and
+// per-frame alignment checks the other launches do not compile in.
+template <bool PREPARED>
 __global__ void __launch_bounds__(kET, kFastEncMinBlocks) encode_xyzi_fast_kernel(const EncLaunch L, const FloatNParams P) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   __shared__ EncFastShared sh;
   __shared__ EncFrame s_F[2];
   __shared__ FloatNParams s_P;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const bool aligned16 = (L.flags & kEncInputsAligned16) != 0u;
+  const bool all_aligned16 = (L.flags & kEncInputsAligned16) != 0u;
+  auto input_aligned16 = [&](const uint8_t* in) { return PREPARED ? enc_input_aligned16(L.flags, in) : all_aligned16; };
 
   if (blockIdx.x == 0) handle_empty_frames(L);
   if (threadIdx.x == 0) {
@@ -176,7 +180,7 @@ __global__ void __launch_bounds__(kET, kFastEncMinBlocks) encode_xyzi_fast_kerne
   // asks for the 1024 points of tile t of frame F into `buf` (transposed slots); false if the tile is not eligible
   auto prefetch = [&](const EncFrame& F, uint32_t tt, uint8_t* buf) -> bool {
     const uint32_t p0 = tt * kETilePts;
-    if (!aligned16 || p0 + kETilePts > F.n_points) return false;
+    if (!input_aligned16(F.in) || p0 + kETilePts > F.n_points) return false;
     const uint4* src = reinterpret_cast<const uint4*>(F.in) + p0 + warp * (32 * kEP) + lane;
     uint4* wsl = reinterpret_cast<uint4*>(buf) + warp * (32 * kEP);
 #pragma unroll
@@ -205,7 +209,7 @@ __global__ void __launch_bounds__(kET, kFastEncMinBlocks) encode_xyzi_fast_kerne
       // (every thread needs the frame's input pointer and size for its own copies: read them from the table directly)
       const EncFrame* NF = L.frames + nfi;
       const uint32_t p0 = nt * kETilePts;
-      if (aligned16 && p0 + kETilePts <= NF->n_points) {
+      if (p0 + kETilePts <= NF->n_points && input_aligned16(NF->in)) {
         const uint4* src = reinterpret_cast<const uint4*>(NF->in) + p0 + warp * (32 * kEP) + lane;
         uint4* wsl = reinterpret_cast<uint4*>(dyn_smem + (cur ^ 1u) * kEBufBytes) + warp * (32 * kEP);
 #pragma unroll
@@ -218,151 +222,159 @@ __global__ void __launch_bounds__(kET, kFastEncMinBlocks) encode_xyzi_fast_kerne
     }
     async_commit();
 
-    const uint32_t tile = F.tile_begin + t;
-    const uint32_t tile_p0 = t * kETilePts;
-    const bool full = tile_p0 + kETilePts <= F.n_points;
-    uint32_t total = 0;
-    bool fast = full;
-    uint32_t X[kEP][4];
-    uint32_t mine = 0, tail4 = 0;
-    if (full) {
-      const uint32_t wp0 = tile_p0 + warp * (32 * kEP);
-      uint4* wsl = reinterpret_cast<uint4*>(buf) + warp * (32 * kEP);
-      if (have_cur) {
-        async_wait_all_but_last();   // this tile's copies have landed (the next tile's may still be in flight)
-      } else {
-        // ---- load + transpose inside the warp: lane l of iteration k loads point 32 k + l of the warp's 256 ----
+    // An empty tile slot (EncLaunch::empty_slots) is left at once; its ticket is drawn like any other. It cannot stall the
+    // look-back: a tile only waits for earlier tiles of its own frame, which are real, and a frame's real tiles come
+    // before its empty slots in ticket order (t < n_tiles <= t'), so they are held by running CTAs as argued above.
+    if (!(PREPARED && t >= F.n_tiles)) {
+      const uint32_t tile = F.tile_begin + t;
+      const uint32_t tile_p0 = t * kETilePts;
+      const bool full = tile_p0 + kETilePts <= F.n_points;
+      const bool aligned16 = input_aligned16(F.in);
+      uint32_t total = 0;
+      bool fast = full;
+      uint32_t X[kEP][4];
+      uint32_t mine = 0, tail4 = 0;
+      if (full) {
+        const uint32_t wp0 = tile_p0 + warp * (32 * kEP);
+        uint4* wsl = reinterpret_cast<uint4*>(buf) + warp * (32 * kEP);
+        if (have_cur) {
+          async_wait_all_but_last();   // this tile's copies have landed (the next tile's may still be in flight)
+        } else {
+          // ---- load + transpose inside the warp: lane l of iteration k loads point 32 k + l of the warp's 256 ----
 #pragma unroll
-        for (int k = 0; k < kEP; ++k) {
-          const uint32_t q = 32u * k + lane;
-          uint4 v;
-          if (aligned16) {
-            v = __ldcs(reinterpret_cast<const uint4*>(F.in) + wp0 + q);
-          } else {
-            const uint8_t* pt = F.in + static_cast<size_t>(wp0 + q) * 16u;
-            v = make_uint4(load_u32(pt), load_u32(pt + 4), load_u32(pt + 8), load_u32(pt + 12));
+          for (int k = 0; k < kEP; ++k) {
+            const uint32_t q = 32u * k + lane;
+            uint4 v;
+            if (aligned16) {
+              v = __ldcs(reinterpret_cast<const uint4*>(F.in) + wp0 + q);
+            } else {
+              const uint8_t* pt = F.in + static_cast<size_t>(wp0 + q) * 16u;
+              v = make_uint4(load_u32(pt), load_u32(pt + 4), load_u32(pt + 8), load_u32(pt + 12));
+            }
+            const uint32_t ol = q >> 3;  // owner lane; slot of point j of lane l: 8 l + (j ^ (l & 7))
+            wsl[8 * ol + ((q & 7u) ^ (ol & 7u))] = v;
           }
-          const uint32_t ol = q >> 3;  // owner lane; slot of point j of lane l: 8 l + (j ^ (l & 7))
-          wsl[8 * ol + ((q & 7u) ^ (ol & 7u))] = v;
         }
-      }
-      // previous point of my first point: 0 at a chunk start, else quantised like any point
-      const uint32_t p_first = wp0 + lane * kEP;
-      uint4 pvu = make_uint4(0, 0, 0, 0);
-      if (lane == 0 && (p_first % kChunkPoints) != 0) {
-        const uint8_t* pt = F.in + static_cast<size_t>(p_first - 1) * 16u;
-        pvu = make_uint4(load_u32(pt), load_u32(pt + 4), load_u32(pt + 8), load_u32(pt + 12));
-      }
-      __syncwarp();
-      if (lane != 0) {
-        const uint32_t pl = lane - 1;
-        pvu = wsl[8 * pl + (7u ^ (pl & 7u))];
-      }
-      float trk = 0.0f;
-      int32_t prev[4];
-      {
-        const float pf[4] = {__uint_as_float(pvu.x), __uint_as_float(pvu.y), __uint_as_float(pvu.z), __uint_as_float(pvu.w)};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float s = __fmul_rn(pf[k], P.mul[k]);
-          trk = max_nan(trk, fabsf(s));
-          prev[k] = __float2int_rn(s);
+        // previous point of my first point: 0 at a chunk start, else quantised like any point
+        const uint32_t p_first = wp0 + lane * kEP;
+        uint4 pvu = make_uint4(0, 0, 0, 0);
+        if (lane == 0 && (p_first % kChunkPoints) != 0) {
+          const uint8_t* pt = F.in + static_cast<size_t>(p_first - 1) * 16u;
+          pvu = make_uint4(load_u32(pt), load_u32(pt + 4), load_u32(pt + 8), load_u32(pt + 12));
         }
-      }
-      // ---- pass 1: LEB128 words of my 32 values + their total length ----
-      uint32_t nbl[3] = {0, 0, 0};  // bit lengths of my last three values (for the tail word)
-#pragma unroll
-      for (int j = 0; j < kEP; ++j) {
-        const uint4 u = wsl[8 * lane + (j ^ (lane & 7))];
-        const float pf[4] = {__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w)};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float s = __fmul_rn(pf[k], P.mul[k]);   // _mm_mul_ps: IEEE RN, never contracted
-          trk = max_nan(trk, fabsf(s));
-          const int32_t q = __float2int_rn(s);          // cvtps2dq under the default MXCSR: ties to even
-          const uint32_t d = static_cast<uint32_t>(q) - static_cast<uint32_t>(prev[k]);
-          prev[k] = q;
-          const uint32_t zz1 = ((d << 1) ^ static_cast<uint32_t>(static_cast<int32_t>(d) >> 31)) + 1u;  // < 2^28 on the fast path
-          // 7-bit groups -> bytes: 14-bit halves into 16-bit lanes, then the upper 7 bits of each lane one bit up
-          uint32_t x = (zz1 & 0xFFFFC000u) * 3u + zz1;           // lo14 + hi14 * 2^16 (one LOP3 + one IMAD)
-          x = x + (x & 0x3F803F80u);
-          const uint32_t b = top_bit(x);                           // inside the value's last byte (garbage tiles: x may be 0)
-          x |= low_mask(b) & 0x00808080u;                          // continuation flags on every byte below it
-          X[j][k] = x;
-          mine += b >> 3;
-          if (j == kEP - 1 && k >= 1) nbl[k - 1] = (b & 0x18u) + 8u;
+        __syncwarp();
+        if (lane != 0) {
+          const uint32_t pl = lane - 1;
+          pvu = wsl[8 * pl + (7u ^ (pl & 7u))];
         }
-      }
-      mine += kEP * 4;
-      // last 4 bytes of my run (top byte = most recent): the successor starts its window with them
-      tail4 = __funnelshift_rc(tail4, X[kEP - 1][1], nbl[0]);
-      tail4 = __funnelshift_rc(tail4, X[kEP - 1][2], nbl[1]);
-      tail4 = __funnelshift_rc(tail4, X[kEP - 1][3], nbl[2]);
-      fast = trk < 33554432.0f;  // 2^25; false for NaN
-    }
-    // ---- offsets: warp scan + warp totals ----
-    uint32_t inc = mine;
+        float trk = 0.0f;
+        int32_t prev[4];
+        {
+          const float pf[4] = {__uint_as_float(pvu.x), __uint_as_float(pvu.y), __uint_as_float(pvu.z), __uint_as_float(pvu.w)};
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t up = __shfl_up_sync(0xffffffffu, inc, d);
-      if (lane >= d) inc += up;
-    }
-    uint32_t ptail = __shfl_up_sync(0xffffffffu, tail4, 1);
-    if (lane == 31) { sh.wtot[warp] = inc; sh.wtail[warp] = tail4; }
-    const int any_slow = __syncthreads_or(fast ? 0 : 1);  // also: every warp is done with its transposed input
-    LookbackPoll lb;
-    if (!any_slow) {
-      uint32_t wbase = 0;
+          for (int k = 0; k < 4; ++k) {
+            const float s = __fmul_rn(pf[k], P.mul[k]);
+            trk = max_nan(trk, fabsf(s));
+            prev[k] = __float2int_rn(s);
+          }
+        }
+        // ---- pass 1: LEB128 words of my 32 values + their total length ----
+        uint32_t nbl[3] = {0, 0, 0};  // bit lengths of my last three values (for the tail word)
 #pragma unroll
-      for (int w = 0; w < kEW; ++w) {
-        const uint32_t c = sh.wtot[w];
-        if (w < warp) wbase += c;
-        total += c;
+        for (int j = 0; j < kEP; ++j) {
+          const uint4 u = wsl[8 * lane + (j ^ (lane & 7))];
+          const float pf[4] = {__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w)};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float s = __fmul_rn(pf[k], P.mul[k]);   // _mm_mul_ps: IEEE RN, never contracted
+            trk = max_nan(trk, fabsf(s));
+            const int32_t q = __float2int_rn(s);          // cvtps2dq under the default MXCSR: ties to even
+            const uint32_t d = static_cast<uint32_t>(q) - static_cast<uint32_t>(prev[k]);
+            prev[k] = q;
+            const uint32_t zz1 = ((d << 1) ^ static_cast<uint32_t>(static_cast<int32_t>(d) >> 31)) + 1u;  // < 2^28 on the fast path
+            // 7-bit groups -> bytes: 14-bit halves into 16-bit lanes, then the upper 7 bits of each lane one bit up
+            uint32_t x = (zz1 & 0xFFFFC000u) * 3u + zz1;           // lo14 + hi14 * 2^16 (one LOP3 + one IMAD)
+            x = x + (x & 0x3F803F80u);
+            const uint32_t b = top_bit(x);                           // inside the value's last byte (garbage tiles: x may be 0)
+            x |= low_mask(b) & 0x00808080u;                          // continuation flags on every byte below it
+            X[j][k] = x;
+            mine += b >> 3;
+            if (j == kEP - 1 && k >= 1) nbl[k - 1] = (b & 0x18u) + 8u;
+          }
+        }
+        mine += kEP * 4;
+        // last 4 bytes of my run (top byte = most recent): the successor starts its window with them
+        tail4 = __funnelshift_rc(tail4, X[kEP - 1][1], nbl[0]);
+        tail4 = __funnelshift_rc(tail4, X[kEP - 1][2], nbl[1]);
+        tail4 = __funnelshift_rc(tail4, X[kEP - 1][3], nbl[2]);
+        fast = trk < 33554432.0f;  // 2^25; false for NaN
       }
-      // the tile's size is final: publish it before the bytes are packed, so that successors never wait for pass 2
+      // ---- offsets: warp scan + warp totals ----
+      uint32_t inc = mine;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t up = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc += up;
+      }
+      uint32_t ptail = __shfl_up_sync(0xffffffffu, tail4, 1);
+      if (lane == 31) { sh.wtot[warp] = inc; sh.wtail[warp] = tail4; }
+      const int any_slow = __syncthreads_or(fast ? 0 : 1);  // also: every warp is done with its transposed input
+      LookbackPoll lb;
+      if (!any_slow) {
+        uint32_t wbase = 0;
+#pragma unroll
+        for (int w = 0; w < kEW; ++w) {
+          const uint32_t c = sh.wtot[w];
+          if (w < warp) wbase += c;
+          total += c;
+        }
+        // the tile's size is final: publish it before the bytes are packed, so that successors never wait for pass 2
+        if (warp == 0) {
+          lb.begin(L.status, F.tile_begin, tile, L.epoch, total);
+          lb.issue(L.status, F.tile_begin, L.epoch);
+        }
+        if (lane == 0) ptail = warp > 0 ? sh.wtail[warp - 1] : 0u;
+        const uint32_t off = wbase + inc - mine;
+        // ---- pass 2: 64-bit window, aligned word flushes ----
+        // `bit` = bit position of the next byte in the tile's stream; the window's low word is the aligned word holding it
+        uint32_t bit = 8u * off;
+        uint32_t lo = __funnelshift_rc(ptail, 0u, 32u - (bit & 31u));   // the last off % 4 bytes of the predecessor (0 if none)
+        uint32_t wa = (bit >> 3) & ~3u;                                 // byte address of that word in the staging buffer
+#pragma unroll
+        for (int j = 0; j < kEP; ++j) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const uint32_t x = X[j][k];
+            const uint32_t b = top_bit(x);
+            lo |= __funnelshift_l(0u, x, bit);                 // x << (bit % 32)
+            const uint32_t hi = __funnelshift_l(x, 0u, bit);   // x >> (32 - bit % 32), 0 for bit % 32 == 0
+            bit += (b & 0x18u) + 8u;
+            const uint32_t wn = (bit >> 3) & ~3u;
+            if (wn != wa) { *reinterpret_cast<uint32_t*>(stage + wa) = lo; lo = hi; }
+            wa = wn;
+          }
+        }
+        if (threadIdx.x == kET - 1 && (bit & 31u) != 0u) *reinterpret_cast<uint32_t*>(stage + wa) = lo;  // nobody follows the tile's last thread
+      } else {
+        // exact path: up to 20 bytes per point, staged from the start of the dynamic shared memory across BOTH input buffers --
+        // the next tile's copies are drained first and the tile is loaded again, synchronously, when its turn comes
+        async_wait_all();
+        __syncthreads();
+        have_next = false;
+        stage = dyn_smem;
+        total = encode_tile_careful<4>(F, s_P, tile_p0, stage, sh.scan);
+        if (warp == 0) lb.begin(L.status, F.tile_begin, tile, L.epoch, total);
+      }
+      // ---- the tile's place in the frame ----
       if (warp == 0) {
-        lb.begin(L.status, F.tile_begin, tile, L.epoch, total);
-        lb.issue(L.status, F.tile_begin, L.epoch);
+        const uint64_t e = lb.finish(L.status, F.tile_begin, tile, L.epoch, total);
+        if (lane == 0) sh.excl = e;
       }
-      if (lane == 0) ptail = warp > 0 ? sh.wtail[warp - 1] : 0u;
-      const uint32_t off = wbase + inc - mine;
-      // ---- pass 2: 64-bit window, aligned word flushes ----
-      // `bit` = bit position of the next byte in the tile's stream; the window's low word is the aligned word holding it
-      uint32_t bit = 8u * off;
-      uint32_t lo = __funnelshift_rc(ptail, 0u, 32u - (bit & 31u));   // the last off % 4 bytes of the predecessor (0 if none)
-      uint32_t wa = (bit >> 3) & ~3u;                                 // byte address of that word in the staging buffer
-#pragma unroll
-      for (int j = 0; j < kEP; ++j) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t x = X[j][k];
-          const uint32_t b = top_bit(x);
-          lo |= __funnelshift_l(0u, x, bit);                 // x << (bit % 32)
-          const uint32_t hi = __funnelshift_l(x, 0u, bit);   // x >> (32 - bit % 32), 0 for bit % 32 == 0
-          bit += (b & 0x18u) + 8u;
-          const uint32_t wn = (bit >> 3) & ~3u;
-          if (wn != wa) { *reinterpret_cast<uint32_t*>(stage + wa) = lo; lo = hi; }
-          wa = wn;
-        }
-      }
-      if (threadIdx.x == kET - 1 && (bit & 31u) != 0u) *reinterpret_cast<uint32_t*>(stage + wa) = lo;  // nobody follows the tile's last thread
+      __syncthreads();  // staged bytes + sh.excl complete (and s_F[cur ^ 1] written)
+      finish_tile<kETilePts>(L, F, fi, t, stage, total, sh.excl);
     } else {
-      // exact path: up to 20 bytes per point, staged from the start of the dynamic shared memory across BOTH input buffers --
-      // the next tile's copies are drained first and the tile is loaded again, synchronously, when its turn comes
-      async_wait_all();
-      __syncthreads();
-      have_next = false;
-      stage = dyn_smem;
-      total = encode_tile_careful<4>(F, s_P, tile_p0, stage, sh.scan);
-      if (warp == 0) lb.begin(L.status, F.tile_begin, tile, L.epoch, total);
+      __syncthreads();  // every thread has read sh.ticket before thread 0 draws the next one
     }
-    // ---- the tile's place in the frame ----
-    if (warp == 0) {
-      const uint64_t e = lb.finish(L.status, F.tile_begin, tile, L.epoch, total);
-      if (lane == 0) sh.excl = e;
-    }
-    __syncthreads();  // staged bytes + sh.excl complete (and s_F[cur ^ 1] written)
-    finish_tile<kETilePts>(L, F, fi, t, stage, total, sh.excl);
     // the ticket for the tile after next is drawn just before that tile's copies are issued
     if (threadIdx.x == 0 && nxt < L.n_tiles_total) sh.ticket = atomicAdd(L.tile_ticket, 1u);
     __syncthreads();  // this buffer receives the tile after next (and sh.ticket is published)
@@ -391,15 +403,10 @@ bool encode_fast_applies(const Plan& plan) {
 }
 uint32_t encode_fast_tile_points() { return kETilePts; }
 
-static int launch_encode_fast(const Plan& plan, const EncLaunch& L, cudaStream_t stream) {
-  FloatNParams P;
-  for (int k = 0; k < 4; ++k) {
-    P.offset[k] = plan.ops[0].offset[k];
-    P.mul[k] = plan.ops[0].enc_mul_f[k];
-  }
-  P.point_step = plan.point_step;
+template <bool PREPARED>
+static int launch_encode_fast_as(const EncLaunch& L, const FloatNParams& P, cudaStream_t stream) {
   const size_t smem = kESmemBytes;
-  auto k = encode_xyzi_fast_kernel;
+  auto k = encode_xyzi_fast_kernel<PREPARED>;
   if (set_smem(k, smem) != cudaSuccess) return -1;
   // persistent grid of one GPU's worth of CTAs; they take their tiles from the ticket counter, so none has to be resident
   static const int resident = [&] {
@@ -414,6 +421,16 @@ static int launch_encode_fast(const Plan& plan, const EncLaunch& L, cudaStream_t
   k<<<grid, kET, smem, stream>>>(L, P);
   count_launch();
   return 1;
+}
+
+static int launch_encode_fast(const Plan& plan, const EncLaunch& L, cudaStream_t stream) {
+  FloatNParams P;
+  for (int k = 0; k < 4; ++k) {
+    P.offset[k] = plan.ops[0].offset[k];
+    P.mul[k] = plan.ops[0].enc_mul_f[k];
+  }
+  P.point_step = plan.point_step;
+  return L.empty_slots ? launch_encode_fast_as<true>(L, P, stream) : launch_encode_fast_as<false>(L, P, stream);
 }
 
 }  // namespace cldn

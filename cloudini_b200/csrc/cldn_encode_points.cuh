@@ -72,6 +72,7 @@ __global__ void __launch_bounds__(kPT) encode_points_fast_kernel(const EncLaunch
   const uint32_t fi = L.uniform_tiles ? blockIdx.x % L.n_frames : find_frame(L.frames, L.n_frames, blockIdx.x);
   const EncFrame F = L.frames[fi];
   const uint32_t t = L.uniform_tiles ? blockIdx.x / L.n_frames : blockIdx.x - F.tile_begin;
+  if (L.empty_slots && t >= F.n_tiles) return;  // an empty tile slot (EncLaunch::empty_slots)
   const uint32_t tile = F.tile_begin + t;
   const uint32_t tile_p0 = t * T;
   const bool full = tile_p0 + T <= F.n_points;
@@ -288,7 +289,8 @@ static int launch_points_nf(const Plan& plan, const EncLaunch& L, const PointsPa
   bool aligned4 = (plan.point_step & 3u) == 0u;
   for (int k = 0; k < NV; ++k) aligned4 = aligned4 && (P.offset[k] & 3u) == 0u;
   // (the shared copy keeps the global misalignment of the tile's first byte modulo 16; with a 4-byte aligned layout and
-  //  16-byte aligned frames every field read is one aligned word)
+  //  16-byte aligned frames every field read is one aligned word; kEncAlignPerFrame launches take the unaligned reads,
+  //  which are right at any alignment)
   aligned4 = aligned4 && (L.flags & kEncInputsAligned16);
   if (aligned4) {
     auto k = encode_points_fast_kernel<NV, EP, true, NF>;

@@ -35,11 +35,18 @@ struct EncLaunch {
   uint64_t* sizes;         // per frame: total bytes written (header included)
   uint32_t* err;
   uint32_t tile_points;    // 256 * I (choose_tile_points)
-  uint32_t flags;          // kEncInputsAligned16: every frame's input base is 16-byte aligned
+  uint32_t flags;          // kEncInputsAligned16 / kEncAlignPerFrame
   uint32_t uniform_tiles;  // > 0: every frame has exactly this many tiles (frame = tile / uniform_tiles, no search)
   uint32_t* tile_ticket;   // one word, zeroed per launch: the persistent XYZI kernel's CTAs take their tiles from it in order
+  uint32_t* frame_err;     // nullptr, or one word per frame that takes that frame's errors (frame_err_word)
+  uint32_t empty_slots;    // 1: every frame owns uniform_tiles tile slots, and the slots t >= n_tiles are empty
 };
-constexpr uint32_t kEncInputsAligned16 = 1u;
+constexpr uint32_t kEncInputsAligned16 = 1u;  // every frame's input base is 16-byte aligned (checked on the host)
+constexpr uint32_t kEncAlignPerFrame = 2u;    // the host has not seen the inputs: each frame's base is checked on the device
+// Whether frame input `in` takes the 16-byte loads.
+__device__ __forceinline__ bool enc_input_aligned16(uint32_t flags, const uint8_t* in) {
+  return (flags & kEncInputsAligned16) || ((flags & kEncAlignPerFrame) && (reinterpret_cast<uintptr_t>(in) & 15u) == 0u);
+}
 uint32_t choose_tile_points(const Plan& plan);
 
 // Interleaved regular stream + chunk framing. Returns the number of kernels launched.
@@ -155,6 +162,8 @@ struct SecLaunch {
   uint64_t* hash_scratch;        // palette hash tables
   uint32_t* err;
   uint32_t header_bytes;
+  uint32_t* frame_err;           // nullptr, or one word per frame (frame_err_word)
+  uint32_t empty_slots;          // 1: chunk slots past a frame's n_chunks are empty, and the kernels leave them at once
 };
 int launch_encode_sections(const Plan& host_plan, const SecLaunch& L, cudaStream_t stream);
 size_t palette_overflow_scratch_bytes();
@@ -193,6 +202,9 @@ struct Lz4Launch {
   // nullptr: one piece per chunk (LZ4).
   const uint32_t* block_begin = nullptr;  // n_chunks_total + 1 entries
   uint32_t n_blocks_total = 0;
+  // compression: 1 when chunk slots past a frame's n_chunks are empty (cldn_b200_encode_blobs_async); decompression
+  // always checks them (chunk_slot_empty)
+  uint32_t empty_slots = 0;
 };
 // Compression: one LZ4 block per chunk, then the blobs are packed (launch_stage2_pack)
 int launch_lz4_compress(const Lz4Launch& L, const uint8_t* header, uint32_t header_bytes, cudaStream_t stream);
@@ -268,6 +280,51 @@ int launch_blobs_async_headers(const AsyncLaunch& A, cudaStream_t stream);
 int launch_blobs_async_link(const AsyncLaunch& A, cudaStream_t stream);
 // status[f] / decoded[f] from the frame's error word.
 int launch_blobs_async_status(const AsyncLaunch& A, cudaStream_t stream);
+
+// ---- device clouds of the encoder's layout, without the host (cldn_b200_encode_blobs_async; cldn_blobs_async.cu) -------
+struct CloudDesc {  // cldn_cloud_desc_t
+  const uint8_t* cloud;
+  uint64_t cloud_bytes;
+  uint8_t* out;
+  uint64_t capacity;
+  uint32_t width, height;
+};
+struct EncAsyncLaunch {
+  const CloudDesc* desc;      // device, n_frames
+  uint32_t n_frames;
+  uint32_t n_tables;          // frames of the prepared shape (>= n_frames): the tables of frames n_frames.. are written empty
+  const uint8_t* tmpl;        // the layout's header with width and height cut out: part 0 | part 1 | part 2 ('\0' included)
+  uint32_t tmpl_len[3];
+  uint32_t point_step;
+  uint64_t max_points;
+  // MaxCompressedSize (without header) of n points: n / kChunkPoints full chunks of full_chunk bytes, and a last chunk of
+  // r = n % kChunkPoints points of 4 + bound(r * per_point + chunk_extra) bytes; bound is the stage-2 worst case of
+  // `compression`. full_chunk_s1 / the NONE bound: the same for the stage-1 arena of the compressed layouts.
+  uint64_t per_point;
+  uint32_t chunk_extra;
+  uint32_t compression;       // CLDN_COMP_* of the blobs
+  uint64_t full_chunk, full_chunk_s1;
+  uint32_t tile_points;
+  uint32_t tiles_per_frame;   // tile slots of a frame (frame f: f * tiles_per_frame ..)
+  uint32_t slots;             // chunk slots of a frame (frame f: f * slots ..)
+  EncFrame* frames;           // stage 1
+  Lz4Frame* lz_frames;        // stage 2 (LZ4 / ZSTD), else nullptr
+  uint8_t* s1;                // stage 2: stage-1 arena of frame f at s1 + f * s1_stride
+  uint64_t s1_stride;
+  uint32_t* sec_excl;         // V5: frame f's (slots + 1) entries at sec_excl + f * (slots + 1), else nullptr
+  uint8_t* side;              // Gorilla records: frame f's at side + f * side_stride, else nullptr
+  uint64_t side_stride;
+  uint64_t* sizes;            // per frame: payload bytes (EncLaunch::sizes, Lz4Launch::sizes)
+  uint32_t* hdr_len;          // per frame: header bytes of a good frame, 0 else
+  uint32_t* frame_err;        // one word per frame, zeroed before the launches
+  uint32_t* err;              // the launches' word (errors no frame claimed)
+  int32_t* status;            // device, n_frames
+  uint64_t* written;          // device, n_frames, optional
+};
+// Frame checks, headers and frame tables; status[f] = CLDN_OK or the refusal.
+int launch_encode_async_frames(const EncAsyncLaunch& A, cudaStream_t stream);
+// status[f] / written[f] from the frame's error word.
+int launch_encode_async_status(const EncAsyncLaunch& A, cudaStream_t stream);
 
 uint64_t kernel_launch_count();
 void count_launch(int n = 1);  // process-wide, atomic: handles on other threads count into the same total

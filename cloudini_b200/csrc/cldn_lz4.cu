@@ -212,6 +212,7 @@ __global__ void __launch_bounds__(kLzThreads) lz4_compress_chunks_kernel(const L
   if (gc >= L.n_chunks_total) return;
   const uint32_t f = L.chunk_frame[gc];
   const Lz4Frame F = L.frames[f];
+  if (L.empty_slots && chunk_slot_empty(F, gc)) return;
   const uint32_t c = gc - F.chunk_begin;
   uint64_t body = 0;
   const uint32_t n = lz_find_chunk(F.plain, *F.plain_bytes, c, &body);
@@ -219,7 +220,7 @@ __global__ void __launch_bounds__(kLzThreads) lz4_compress_chunks_kernel(const L
   if (n != 0xFFFFFFFFu) csize = lz4_compress_warp(F.plain + body, n, L.scratch + static_cast<size_t>(gc) * L.slot_stride, L.slot_stride, s_table[warp]);
   if (lane == 0) {
     L.chunk_sizes[gc] = csize;
-    if (csize == 0u) report_error(L.err, DEV_ERR_LZ4);  // cannot happen with slots of LZ4_COMPRESSBOUND size
+    if (csize == 0u) report_frame_error(L, f, DEV_ERR_LZ4);  // cannot happen with slots of LZ4_COMPRESSBOUND size
   }
 }
 
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(256) lz4_pack_frames_kernel(const Lz4Launch L,
   if (threadIdx.x == 0) {
     s_pos = pos;
     L.sizes[f] = fits ? pos : 0ull;
-    if (!fits) report_error(to_blob ? L.err : frame_err_word(L, f), to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : unpack_err);
+    if (!fits) report_frame_error(L, f, to_blob ? DEV_ERR_ENCODE_OUTPUT_SMALL : unpack_err);
   }
   (void)s_pos;
 }

@@ -439,6 +439,7 @@ __global__ void __launch_bounds__(kSecThreads, 1) encode_sections_kernel(const S
   const uint32_t f = L.chunk_frame[gc];
   const EncFrame F = L.frames[f];
   const uint32_t chunk = gc - L.chunk_first[f];
+  if (L.empty_slots && chunk >= F.n_chunks) return;
   const SecItem it = make_item(F, plan, chunk, s);
   uint8_t* out = L.scratch + static_cast<size_t>(blockIdx.x) * L.sec_stride;
   const uint8_t mode = L.modes[f * ns + s];
@@ -683,6 +684,7 @@ __global__ void __launch_bounds__(kSecThreads, 1) encode_sections_staged_kernel(
   const uint32_t f = L.chunk_frame[gc];
   const EncFrame F = L.frames[f];
   const uint32_t chunk = gc - L.chunk_first[f];
+  if (L.empty_slots && chunk >= F.n_chunks) return;
   const SecItem src = make_item(F, plan, chunk, s);
   const bool is_signed = src.type == CLDN_INT8 || src.type == CLDN_INT16 || src.type == CLDN_INT32;
   const uint32_t ext_shift = 32u - 8u * src.bpv;
@@ -734,6 +736,7 @@ __global__ void __launch_bounds__(kSecThreads, 1) palette_overflow_kernel(const 
     const uint32_t gc = item / ns, s = item % ns;
     const uint32_t f = L.chunk_frame[gc];
     const EncFrame F = L.frames[f];
+    if (L.empty_slots && gc - L.chunk_first[f] >= F.n_chunks) continue;  // (an empty slot's size word is never written)
     const SecItem it = make_item(F, plan, gc - L.chunk_first[f], s);
     uint8_t* out = L.scratch + static_cast<size_t>(item) * L.sec_stride;
     const uint32_t size = write_palette_section(T, it, out, sh.idx16, &sh.count, sh.scan);
@@ -780,6 +783,7 @@ __global__ void __launch_bounds__(kThreads) place_sections_kernel(const SecLaunc
   const uint32_t f = L.chunk_frame[gc];
   const EncFrame F = L.frames[f];
   const uint32_t chunk = gc - L.chunk_first[f];
+  if (L.empty_slots && chunk >= F.n_chunks) return;
   const uint32_t tiles_per_chunk = kChunkPoints / tile_points;
   uint32_t last_tile = (chunk + 1) * tiles_per_chunk - 1;
   if (last_tile >= F.n_tiles) last_tile = F.n_tiles - 1;
@@ -790,7 +794,7 @@ __global__ void __launch_bounds__(kThreads) place_sections_kernel(const SecLaunc
   const uint8_t* src = L.scratch + static_cast<size_t>(blockIdx.x) * L.sec_stride;
   uint8_t* dst = F.out + pos;
   if (pos + size > F.out_cap) {  // the reference: "Output buffer too small for uncompressed chunk" (chunk_writer.cpp:33-35)
-    if (threadIdx.x == 0) report_error(L.err, DEV_ERR_ENCODE_OUTPUT_SMALL);
+    if (threadIdx.x == 0) report_frame_error(L, f, DEV_ERR_ENCODE_OUTPUT_SMALL);
     return;
   }
   // through shared memory in 16 KB pieces: 16-byte loads from the (aligned) scratch slot, 16-byte stores at whatever alignment

@@ -291,7 +291,9 @@ __global__ void __launch_bounds__(kZeThreads) zstd_compress_blocks_kernel(const 
     else hi = mid;
   }
   const uint32_t gc = lo, k = b - L.block_begin[gc], allotted = L.block_begin[gc + 1u] - L.block_begin[gc];
-  const Lz4Frame F = L.frames[L.chunk_frame[gc]];
+  const uint32_t f = L.chunk_frame[gc];
+  const Lz4Frame F = L.frames[f];
+  if (L.empty_slots && chunk_slot_empty(F, gc)) return;
   uint64_t body = 0;
   const uint32_t s = lz_find_chunk(F.plain, *F.plain_bytes, gc - F.chunk_begin, &body);
   const uint32_t nblk = s == 0xFFFFFFFFu ? 0u : max(1u, (s + kZeBlock - 1u) / kZeBlock);
@@ -300,7 +302,7 @@ __global__ void __launch_bounds__(kZeThreads) zstd_compress_blocks_kernel(const 
     if (tid == 0) {
       L.chunk_sizes[b] = 0u;
       // (a stage-1 chunk that is not where the chunk table says, or larger than its worst case: cannot happen)
-      if (k == 0u && (s == 0xFFFFFFFFu || nblk > allotted)) report_error(L.err, DEV_ERR_ENCODE_OUTPUT_SMALL);
+      if (k == 0u && (s == 0xFFFFFFFFu || nblk > allotted)) report_frame_error(L, f, DEV_ERR_ENCODE_OUTPUT_SMALL);
     }
     return;
   }

@@ -320,6 +320,47 @@ int cldn_b200_decoder_prepare_blobs(cldn_decoder_t* dec, const cldn_info_t* layo
                                     uint64_t max_points_per_frame);
 int cldn_b200_decode_blobs_async(cldn_decoder_t* dec, size_t n_frames, const void* d_frames, int32_t* d_status,
                                  uint64_t* d_decoded_bytes);
+/* The encode counterpart: device-resident clouds of the ENCODER's layout and any point counts, encoded into complete
+ * device blobs without the host, for producers whose clouds are made on the GPU (filtered, cropped, simulated) and whose
+ * point counts may be known only there, and for callers that capture the encode in a CUDA graph.
+ *
+ * cldn_b200_encoder_prepare_blobs: once per shape, outside any capture. Stage 2 is the handle's setting at this call:
+ * NONE, LZ4 (device coder), or ZSTD only after cldn_b200_encoder_set_stage2_on_device(enc, 1) (otherwise
+ * CLDN_ERR_UNSUPPORTED, as cldn_b200_encode_blobs refuses ZSTD with CLDN_MEM_DEVICE). Uploads the header template and
+ * the shape's tables, and allocates every device buffer a call of up to `max_frames` frames of up to
+ * `max_points_per_frame` points needs, apart from the handle's other scratch. Refuses max_frames == 0 or >= 2^31
+ * (CLDN_ERR_INVALID_ARGUMENT), max_points_per_frame >= 2^32 and shapes with 2^31 tiles or chunks or more
+ * (CLDN_ERR_UNSUPPORTED). A new prepare replaces the previous state; graphs captured before it are then invalid.
+ * cldn_b200_encode, _encode_batch, _encode_blobs and _encoder_set_dims keep working and do not disturb the prepared
+ * state; cldn_b200_encoder_set_stage2_on_device applies from the next prepare.
+ *
+ * cldn_b200_encode_blobs_async: enqueues on the handle's stream and returns. No synchronisation, allocation, pageable
+ * copy or host->device copy, and launches and grids that depend neither on n_frames nor on the point counts.
+ * `d_frames`: DEVICE array of n_frames cldn_cloud_desc_t. d_status (int32 per frame) and d_written (uint64 per frame,
+ * optional: the blob size, header included, 0 for a failed frame) are DEVICE arrays. Returns CLDN_ERR_INVALID_ARGUMENT,
+ * before anything is enqueued, without a prepared shape, with n_frames > max_frames, or with d_frames or d_status NULL.
+ * A good frame's blob is byte-identical to that frame's cldn_b200_encode_blobs alone on this handle (same width and
+ * height, same stage-2 setting). d_status[f] is the status cldn_b200_encode_blobs gives that frame alone:
+ *   CLDN_ERR_INVALID_ARGUMENT  cloud_bytes not a multiple of point_step, a NULL cloud (points > 0) or output, or
+ *                              width * height != points;
+ *   CLDN_ERR_BUFFER_TOO_SMALL  capacity below MaxCompressedSize + the frame's header, or a committed V5 mode that
+ *                              overflows a capacity that passed that check;
+ * and, checked last, the one refusal of this call alone:
+ *   CLDN_ERR_UNSUPPORTED       more points than max_points_per_frame.
+ * A frame refused before the encode writes no byte of its output; a frame that fails during the encode may leave any
+ * bytes in [0, capacity). No byte outside [0, capacity) is written, nor any output of the frames >= n_frames. There are
+ * no messages: encode a failed frame with cldn_b200_encode_blobs for the message. */
+typedef struct cldn_cloud_desc_t {
+  const void* cloud;
+  uint64_t cloud_bytes;
+  void* out;
+  uint64_t capacity;
+  uint32_t width;  /* width = height = 0: (points, 1) */
+  uint32_t height;
+} cldn_cloud_desc_t;
+int cldn_b200_encoder_prepare_blobs(cldn_encoder_t* enc, size_t max_frames, uint64_t max_points_per_frame);
+int cldn_b200_encode_blobs_async(cldn_encoder_t* enc, size_t n_frames, const void* d_frames, int32_t* d_status,
+                                 uint64_t* d_written);
 /* Message of frame f of this handle's last cldn_b200_decode_blobs ("" when it decoded). */
 const char* cldn_b200_decoder_frame_error(const cldn_decoder_t* dec, size_t f);
 /* EncodingInfo read from the header of frame f of this handle's last cldn_b200_decode_blobs (zeroed when the header
