@@ -23,6 +23,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -78,6 +79,10 @@ struct VizLaunch {
   uint32_t* kept;                // per cloud: number of survivors
 };
 
+// Table slots of a cloud of n points: a multiple of 1024 that is at least 2n (load factor <= 1/2). The output does not
+// depend on the size or the hash, only on the table holding every distinct voxel.
+__host__ __device__ __forceinline__ uint32_t viz_table_size(uint32_t n) { return ((2u * n + 1023u) / 1024u) * 1024u; }
+
 // Last cloud whose first block (tile) is <= b: empty clouds share their first block with the next one.
 template <uint32_t VizFrame::*Begin>
 __device__ __forceinline__ uint32_t find_viz_frame(const VizFrame* __restrict__ frames, uint32_t n_frames, uint32_t b) {
@@ -124,6 +129,8 @@ __global__ void __launch_bounds__(kThreads) viz_compact_kernel(VizLaunch L) {
   const uint32_t tile_points = kThreads * L.ppt;
   const uint32_t n = F.n_points;
   const uint32_t tile = blockIdx.x - F.tile_begin;
+  // a tile slot past the cloud's last tile (the prepared grid of the async call) joins no look-back and writes no count
+  if (static_cast<uint64_t>(tile) * tile_points >= n) return;
   const uint32_t* slots = L.slots + F.slot_base;
   const uint32_t* firsts = L.firsts + F.table_base;
   const uint8_t* in = F.in;
@@ -180,6 +187,106 @@ __global__ void __launch_bounds__(kThreads) viz_compact_kernel(VizLaunch L) {
   }
 }
 
+// ---- device clouds of one prepared layout, without the host (cldn_b200_viz_lossy_preprocess_batch_async) ------------
+// Every frame slot f of the prepared shape owns blocks [f * blocks_per_frame, ..), tiles [f * tiles_per_frame, ..), the
+// table region [f * table_per_frame, ..) and the slots [f * max_points, ..), so the insert and compact grids are those of
+// max_frames clouds of max_points points whatever the call holds. The frame kernel writes the frame table on the device;
+// a frame that is not rewritten (refused, empty, no-op, or past n_frames) gets n_points = 0, and all its blocks and
+// tiles leave at once.
+struct VizDesc {  // cldn_viz_desc_t
+  const uint8_t* cloud;
+  uint64_t cloud_bytes;
+  uint8_t* out;
+  uint64_t capacity;
+};
+
+struct VizAsyncLaunch {
+  const VizDesc* desc;           // device, n_frames
+  uint32_t n_frames;
+  uint32_t n_slots;              // prepared frames (>= n_frames): the frame table has this many entries
+  uint32_t point_step, xyz_offset;
+  uint32_t noop;                 // the layout is one of the reference's early returns
+  uint32_t max_points;
+  uint32_t blocks_per_frame, tiles_per_frame, table_per_frame, clear_blocks_per_frame;
+  VizFrame* frames;
+  int32_t* frame_status;         // per frame slot: the status the frame kernel decided
+  const uint32_t* kept;          // per frame slot: survivors, written by the compaction's last tile
+  unsigned long long* keys;
+  uint32_t* firsts;
+  // the call's outputs (device, n_frames entries)
+  int32_t* status;
+  uint64_t* kept_out;
+  int32_t* applied;
+  CloudDesc* encode;
+};
+
+constexpr uint32_t kVizClearSlots = 4096;  // table slots cleared per CTA
+
+// One thread per frame slot: the per-frame checks of viz_frames in its order, then the prepared maximum.
+__global__ void __launch_bounds__(kThreads) viz_async_frames_kernel(const VizAsyncLaunch A) {
+  const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+  if (f >= A.n_slots) return;
+  VizDesc D = {nullptr, 0, nullptr, 0};
+  if (f < A.n_frames) D = A.desc[f];
+  const uint64_t n = A.point_step ? D.cloud_bytes / A.point_step : 0;
+  int32_t st = !D.cloud && D.cloud_bytes ? CLDN_ERR_INVALID_ARGUMENT : CLDN_OK;
+  const bool rewritten = st == CLDN_OK && !A.noop && n > 0;  // a no-op layout or an empty cloud is left as it is
+  if (rewritten) {
+    if (n > (1ull << 30)) st = CLDN_ERR_UNSUPPORTED;
+    else if (static_cast<uint64_t>(A.xyz_offset) + 12u > A.point_step) st = CLDN_ERR_INVALID_ARGUMENT;
+    else if (!D.out || D.capacity < n * A.point_step) st = CLDN_ERR_BUFFER_TOO_SMALL;
+    else if (n > A.max_points) st = CLDN_ERR_UNSUPPORTED;  // the one refusal of the async call alone
+  }
+  const uint32_t pts = rewritten && st == CLDN_OK ? static_cast<uint32_t>(n) : 0u;
+  VizFrame F;
+  F.in = D.cloud;
+  F.out = D.out;
+  F.n_points = pts;
+  F.block_begin = f * A.blocks_per_frame;
+  F.tile_begin = f * A.tiles_per_frame;
+  F.table_size = pts ? viz_table_size(pts) : 0u;
+  F.table_base = static_cast<uint64_t>(f) * A.table_per_frame;
+  F.slot_base = static_cast<uint64_t>(f) * A.max_points;
+  A.frames[f] = F;
+  A.frame_status[f] = st;
+}
+
+// keys = kEmptyVoxel and firsts = ~0 over [0, table_size) of every rewritten frame: the bytes cleared follow the
+// frames' points, not the prepared maximum. table_size and the region bases are multiples of 1024 slots.
+__global__ void __launch_bounds__(kThreads) viz_clear_kernel(const VizAsyncLaunch A) {
+  const uint32_t f = blockIdx.x / A.clear_blocks_per_frame;
+  const uint32_t begin = (blockIdx.x - f * A.clear_blocks_per_frame) * kVizClearSlots;
+  const VizFrame F = A.frames[f];
+  if (begin >= F.table_size) return;
+  const uint32_t slots = min(kVizClearSlots, F.table_size - begin);
+  const uint4 ones = make_uint4(~0u, ~0u, ~0u, ~0u);
+  uint4* keys = reinterpret_cast<uint4*>(A.keys + F.table_base + begin);
+  for (uint32_t i = threadIdx.x; i < slots / 2; i += kThreads) keys[i] = ones;
+  uint4* firsts = reinterpret_cast<uint4*>(A.firsts + F.table_base + begin);
+  for (uint32_t i = threadIdx.x; i < slots / 4; i += kThreads) firsts[i] = ones;
+}
+
+// One thread per frame of the call: status, kept, applied and the encoder's descriptor, from the frame table and the
+// survivor counts.
+__global__ void __launch_bounds__(kThreads) viz_async_finish_kernel(const VizAsyncLaunch A) {
+  const uint32_t f = blockIdx.x * kThreads + threadIdx.x;
+  if (f >= A.n_frames) return;
+  const VizDesc D = A.desc[f];
+  const int32_t st = A.frame_status[f];
+  const bool applied = A.frames[f].n_points != 0u;
+  const uint64_t kept = applied ? A.kept[f] : A.point_step ? D.cloud_bytes / A.point_step : 0;
+  A.status[f] = st;
+  if (A.kept_out) A.kept_out[f] = kept;
+  if (A.applied) A.applied[f] = applied ? 1 : 0;
+  if (A.encode) {  // cloud, cloud_bytes, width and height only: out and capacity are the caller's
+    CloudDesc* E = A.encode + f;
+    E->cloud = st != CLDN_OK ? nullptr : applied ? D.out : D.cloud;
+    E->cloud_bytes = st != CLDN_OK ? 1u : applied ? kept * A.point_step : D.cloud_bytes;
+    E->width = 0;
+    E->height = 0;
+  }
+}
+
 }  // namespace cldn
 
 using namespace cldn;
@@ -218,10 +325,67 @@ struct PinnedBuf {
   void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
 
-// Table slots of a cloud of n points: a multiple of 1024 that is at least 2n (load factor <= 1/2). The output does not
-// depend on the size or the hash, only on the table holding every distinct voxel.
-uint32_t viz_table_size(uint32_t n) { return ((2u * n + 1023u) / 1024u) * 1024u; }
+// The reference's early returns that depend on the layout alone (ros_msg_utils.cpp:250-278): true when the layout has no
+// xyz triple or a resolution that is not positive and finite, in which case every cloud of it is left as it is.
+bool viz_noop_layout(const cldn_info_t& info, uint32_t* xyz_offset, float* xyz_res) {
+  *xyz_offset = 0;
+  *xyz_res = 0.0f;
+  if (info.n_fields < 3 || info.point_step == 0) return true;
+  const cldn_field_t &f0 = info.fields[0], &f1 = info.fields[1], &f2 = info.fields[2];
+  const bool has_triple = f0.type == CLDN_FLOAT32 && f1.type == CLDN_FLOAT32 && f2.type == CLDN_FLOAT32 && f0.has_resolution &&
+                          f1.has_resolution && f2.has_resolution && f0.resolution == f1.resolution &&
+                          f0.resolution == f2.resolution && f1.offset == f0.offset + 4u && f2.offset == f0.offset + 8u;
+  *xyz_res = f0.resolution;
+  *xyz_offset = f0.offset;
+  return !has_triple || !(*xyz_res > 0.0f) || !isfinite(*xyz_res);
+}
+
+// Compaction tiles of kThreads x ppt points; staged: the survivors of a tile are gathered in shared memory.
+void viz_tiling(uint32_t step, uint32_t* ppt, bool* staged) {
+  uint32_t p = 8;
+  while (p > 1 && static_cast<size_t>(kThreads) * p * step > (64u << 10)) p >>= 1;
+  *ppt = p;
+  *staged = static_cast<size_t>(kThreads) * p * step <= (200u << 10);
+}
+
+// pc_info bookkeeping of an applied cloud (:327-340), apart from width and height
+void viz_info_after(cldn_info_t* o) {
+  for (uint32_t i = 0; i < o->n_fields; ++i) {
+    if (o->fields[i].type == CLDN_FLOAT64 && !o->fields[i].has_resolution) {
+      o->fields[i].has_resolution = 1;
+      o->fields[i].resolution = 1e-6f;
+    }
+  }
+}
+
+// Device memory of exactly n elements, freed with its owner.
+template <typename T>
+struct DevArray {
+  T* p = nullptr;
+  DevArray() = default;
+  DevArray(const DevArray&) = delete;
+  DevArray& operator=(const DevArray&) = delete;
+  ~DevArray() { if (p) cudaFree(p); }
+  bool alloc(size_t n) { return cudaMalloc(reinterpret_cast<void**>(&p), std::max<size_t>(n, 1) * sizeof(T)) == cudaSuccess; }
+};
 }  // namespace
+
+// The prepared state of cldn_b200_viz_lossy_preprocess_batch_async: separate from the buffers of the single and batch
+// calls, so that those keep working between async calls and a captured graph stays valid until the next prepare.
+struct VizAsync {
+  size_t max_frames = 0;
+  uint32_t ppt = 1;
+  bool staged = false;
+  size_t smem = 0;
+  uint32_t insert_blocks = 0, compact_tiles = 0, clear_blocks = 0;
+  DevArray<uint8_t> table;  // keys (8 B per slot) of every frame's region, then firsts (4 B per slot)
+  DevArray<uint32_t> slots, kept;
+  DevArray<uint64_t> status;
+  DevArray<VizFrame> frames;
+  DevArray<int32_t> frame_status;
+  VizAsyncLaunch A{};  // all but the call's arrays
+  VizLaunch L{};
+};
 
 struct cldn_preproc {
   int device = 0;
@@ -235,6 +399,7 @@ struct cldn_preproc {
   Buf<uint8_t> d_in, d_out;
   PinnedBuf<VizFrame> h_frames;
   PinnedBuf<uint32_t> h_kept;
+  std::unique_ptr<VizAsync> async;  // cldn_b200_preproc_prepare_batch
 };
 
 #define PP_CUDA(expr)                                                                                          \
@@ -258,18 +423,9 @@ static int viz_frames(cldn_preproc_t* pp, const cldn_info_t* info, size_t n_fram
     if (infos_out) infos_out[f] = *info;
   }
   // ---- the reference's early returns: nothing is modified (ros_msg_utils.cpp:250-278) ----
-  bool noop = info->n_fields < 3 || info->point_step == 0;
   float xyz_res = 0.0f;
   uint32_t xyz_offset = 0;
-  if (!noop) {
-    const cldn_field_t &f0 = info->fields[0], &f1 = info->fields[1], &f2 = info->fields[2];
-    const bool has_triple = f0.type == CLDN_FLOAT32 && f1.type == CLDN_FLOAT32 && f2.type == CLDN_FLOAT32 && f0.has_resolution &&
-                            f1.has_resolution && f2.has_resolution && f0.resolution == f1.resolution &&
-                            f0.resolution == f2.resolution && f1.offset == f0.offset + 4u && f2.offset == f0.offset + 8u;
-    xyz_res = f0.resolution;
-    xyz_offset = f0.offset;
-    noop = !has_triple || !(xyz_res > 0.0f) || !isfinite(xyz_res);
-  }
+  const bool noop = viz_noop_layout(*info, &xyz_offset, &xyz_res);
   auto fail = [&](size_t f, int rc, const char* msg) {
     if (name_frames) set_error("frame %zu: %s", f, msg);
     else set_error("%s", msg);
@@ -277,9 +433,9 @@ static int viz_frames(cldn_preproc_t* pp, const cldn_info_t* info, size_t n_fram
   };
   const uint32_t step = info->point_step;
   uint64_t total_points = 0, blocks = 0, tiles = 0, table = 0;
-  uint32_t ppt = 8;
-  while (ppt > 1 && static_cast<size_t>(kThreads) * ppt * step > (64u << 10)) ppt >>= 1;
-  const bool staged = static_cast<size_t>(kThreads) * ppt * step <= (200u << 10);
+  uint32_t ppt;
+  bool staged;
+  viz_tiling(step, &ppt, &staged);
   const uint32_t tile_points = kThreads * ppt;
   for (size_t f = 0; f < n_frames; ++f) {
     if (!clouds[f] && cloud_bytes[f]) return fail(f, CLDN_ERR_INVALID_ARGUMENT, "null argument");
@@ -380,15 +536,124 @@ static int viz_frames(cldn_preproc_t* pp, const cldn_info_t* info, size_t n_fram
       cldn_info_t& o = infos_out[f];
       o.width = static_cast<uint32_t>(kept);
       o.height = 1;
-      for (uint32_t i = 0; i < o.n_fields; ++i) {
-        if (o.fields[i].type == CLDN_FLOAT64 && !o.fields[i].has_resolution) {
-          o.fields[i].has_resolution = 1;
-          o.fields[i].resolution = 1e-6f;
-        }
-      }
+      viz_info_after(&o);
     }
   }
   if (copied) PP_CUDA(cudaStreamSynchronize(pp->stream));
+  return CLDN_OK;
+}
+
+static int prepare_batch_impl(cldn_preproc_t* pp, const cldn_info_t* info, size_t max_frames, uint64_t max_points,
+                              cldn_info_t* info_after) {
+  if (!pp || !info) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_frames == 0 || max_frames > 0x7FFFFFFFull) { set_error("max_frames must be 1 .. 2^31 - 1"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (max_points > (1u << 30)) { set_error("viz preprocessing: more than 2^30 points in one cloud"); return CLDN_ERR_UNSUPPORTED; }
+  float xyz_res = 0.0f;
+  uint32_t xyz_offset = 0;
+  const bool noop = viz_noop_layout(*info, &xyz_offset, &xyz_res);
+  const uint32_t step = info->point_step;
+  uint32_t ppt;
+  bool staged;
+  viz_tiling(step, &ppt, &staged);
+  const uint64_t points = std::max<uint64_t>(max_points, 1), tile_points = static_cast<uint64_t>(kThreads) * ppt;
+  const uint64_t blocks_per_frame = (points + kThreads - 1) / kThreads, tiles_per_frame = (points + tile_points - 1) / tile_points;
+  const uint32_t table_per_frame = viz_table_size(static_cast<uint32_t>(points));
+  const uint32_t clear_per_frame = (table_per_frame + kVizClearSlots - 1) / kVizClearSlots;
+  if (!noop && (max_frames * blocks_per_frame > 0x7FFFFFFFull || max_frames * tiles_per_frame > 0x7FFFFFFFull)) {
+    set_error("max_frames * blocks or tiles per frame must be below 2^31");
+    return CLDN_ERR_UNSUPPORTED;
+  }
+  PP_CUDA(cudaSetDevice(pp->device));
+  PP_CUDA(cudaStreamSynchronize(pp->stream));  // kernels of an earlier prepared state may still read it
+  pp->async.reset();
+  std::unique_ptr<VizAsync> a(new VizAsync());
+  a->max_frames = max_frames;
+  const size_t table_slots = noop ? 0 : max_frames * table_per_frame;
+  if (!a->frames.alloc(max_frames) || !a->frame_status.alloc(max_frames) || !a->kept.alloc(max_frames) ||
+      !a->table.alloc(table_slots * 12) || !a->slots.alloc(noop ? 0 : max_frames * points) ||
+      !a->status.alloc(noop ? 0 : max_frames * tiles_per_frame)) {
+    set_error("device allocation failed");
+    return CLDN_ERR_CUDA;
+  }
+  VizAsyncLaunch& A = a->A;
+  A.n_slots = static_cast<uint32_t>(max_frames);
+  A.point_step = step;
+  A.xyz_offset = xyz_offset;
+  A.noop = noop ? 1u : 0u;
+  A.max_points = static_cast<uint32_t>(max_points);
+  A.blocks_per_frame = static_cast<uint32_t>(blocks_per_frame);
+  A.tiles_per_frame = static_cast<uint32_t>(tiles_per_frame);
+  A.table_per_frame = table_per_frame;
+  A.clear_blocks_per_frame = clear_per_frame;
+  A.frames = a->frames.p;
+  A.frame_status = a->frame_status.p;
+  A.kept = a->kept.p;
+  A.keys = reinterpret_cast<unsigned long long*>(a->table.p);
+  A.firsts = reinterpret_cast<uint32_t*>(a->table.p + table_slots * 8);
+  if (!noop) {
+    a->ppt = ppt;
+    a->staged = staged;
+    a->smem = staged ? static_cast<size_t>(tile_points) * step + 32 : 0;
+    a->insert_blocks = static_cast<uint32_t>(max_frames * blocks_per_frame);
+    a->compact_tiles = static_cast<uint32_t>(max_frames * tiles_per_frame);
+    a->clear_blocks = static_cast<uint32_t>(max_frames * clear_per_frame);
+    PP_CUDA(raise_smem_limit(viz_compact_kernel, a->smem));
+    VizLaunch& L = a->L;
+    L.frames = a->frames.p;
+    L.n_frames = static_cast<uint32_t>(max_frames);
+    L.point_step = step;
+    L.xyz_offset = xyz_offset;
+    L.inv_res = 1.0f / xyz_res;
+    L.keys = A.keys;
+    L.firsts = A.firsts;
+    L.slots = a->slots.p;
+    L.status = a->status.p;
+    L.epoch = 1;  // the words are cleared in every call
+    L.ppt = ppt;
+    L.staged = staged ? 1u : 0u;
+    L.kept = a->kept.p;
+  }
+  if (info_after) {
+    *info_after = *info;
+    if (!noop) {
+      info_after->width = info_after->height = 0;
+      viz_info_after(info_after);
+    }
+  }
+  pp->async = std::move(a);
+  return CLDN_OK;
+}
+
+// Enqueues only. The launches and their grids are those of the prepared layout and shape, whatever the frames: a clear
+// of the tile status words, the frame kernel, the table clear, insert and compact, the finish kernel (frame and finish
+// kernels alone for a no-op layout).
+static int preprocess_batch_async_impl(cldn_preproc_t* pp, size_t n, const void* d_frames, int32_t* d_status, uint64_t* d_kept,
+                                       int32_t* d_applied, cldn_cloud_desc_t* d_encode) {
+  if (!pp) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  VizAsync* a = pp->async.get();
+  if (!a) { set_error("no prepared layout: call cldn_b200_preproc_prepare_batch first"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n > a->max_frames) { set_error("%zu frames: the shape was prepared for at most %zu", n, a->max_frames); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (!d_frames || !d_status) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  if (n == 0) return CLDN_OK;
+  PP_CUDA(cudaSetDevice(pp->device));
+  VizAsyncLaunch A = a->A;
+  A.desc = static_cast<const VizDesc*>(d_frames);
+  A.n_frames = static_cast<uint32_t>(n);
+  A.status = d_status;
+  A.kept_out = d_kept;
+  A.applied = d_applied;
+  A.encode = reinterpret_cast<CloudDesc*>(d_encode);
+  const uint32_t frame_blocks = static_cast<uint32_t>((a->max_frames + kThreads - 1) / kThreads);
+  if (!A.noop) PP_CUDA(cudaMemsetAsync(a->status.p, 0, static_cast<size_t>(a->compact_tiles) * sizeof(uint64_t), pp->stream));
+  viz_async_frames_kernel<<<frame_blocks, kThreads, 0, pp->stream>>>(A);
+  if (!A.noop) {
+    viz_clear_kernel<<<a->clear_blocks, kThreads, 0, pp->stream>>>(A);
+    viz_insert_kernel<<<a->insert_blocks, kThreads, 0, pp->stream>>>(a->L);
+    viz_compact_kernel<<<a->compact_tiles, kThreads, a->smem, pp->stream>>>(a->L);
+  }
+  viz_async_finish_kernel<<<frame_blocks, kThreads, 0, pp->stream>>>(A);
+  count_launch(A.noop ? 2 : 5);
+  PP_CUDA(cudaGetLastError());
   return CLDN_OK;
 }
 
@@ -430,6 +695,7 @@ void cldn_b200_preproc_destroy(cldn_preproc_t* pp) {
   pp->table.release(); pp->slots.release(); pp->kept.release(); pp->status.release(); pp->frames.release();
   pp->d_in.release(); pp->d_out.release();
   pp->h_frames.release(); pp->h_kept.release();
+  pp->async.reset();
   if (pp->own_stream && pp->stream) cudaStreamDestroy(pp->stream);
   delete pp;
 }
@@ -469,6 +735,28 @@ int cldn_b200_viz_lossy_preprocess_batch(cldn_preproc_t* pp, const cldn_info_t* 
     set_error("out of memory");
     return CLDN_ERR_INTERNAL;
   }
+}
+
+int cldn_b200_preproc_prepare_batch(cldn_preproc_t* pp, const cldn_info_t* info, size_t max_frames, uint64_t max_points_per_frame,
+                                    cldn_info_t* info_after) {
+  try {
+    return prepare_batch_impl(pp, info, max_frames, max_points_per_frame, info_after);
+  } catch (const std::bad_alloc&) {
+    set_error("out of memory");
+    return CLDN_ERR_INTERNAL;
+  }
+}
+
+int cldn_b200_viz_lossy_preprocess_batch_async(cldn_preproc_t* pp, size_t n_frames, const void* d_frames, int32_t* d_status,
+                                               uint64_t* d_kept, int32_t* d_applied, cldn_cloud_desc_t* d_encode) {
+  return preprocess_batch_async_impl(pp, n_frames, d_frames, d_status, d_kept, d_applied, d_encode);
+}
+
+int cldn_b200_preproc_sync(cldn_preproc_t* pp) {
+  if (!pp) { set_error("null argument"); return CLDN_ERR_INVALID_ARGUMENT; }
+  PP_CUDA(cudaSetDevice(pp->device));
+  PP_CUDA(cudaStreamSynchronize(pp->stream));
+  return CLDN_OK;
 }
 
 }  // extern "C"

@@ -15,11 +15,12 @@ from typing import Dict, List, Optional
 import numpy as np
 
 from . import (CLDN_MAX_FIELDS, MEM_DEVICE, MEM_HOST, CompressionOption, EncodingInfo, EncodingOptions, FieldType,
-               PointcloudDecoder, PointcloudEncoder, PointField, _CField, _CInfo, _check, _from_c, _to_c, lib)
+               PointcloudDecoder, PointcloudEncoder, PointField, _CField, _CInfo, _check, _from_c, _to_c, blob_descs, lib,
+               pack_blob_descs)
 
 __all__ = ["RosPointCloud2", "getDeserializedPointCloudMessage", "applyResolutionProfile", "toEncodingInfo",
            "convertPointCloud2ToCompressedCloud", "convertCompressedCloudToPointCloud2", "applyVizLossyPreprocessing",
-           "VizPreprocessor"]
+           "VizPreprocessor", "viz_descs", "pack_viz_descs"]
 
 
 class _CRosMsg(C.Structure):
@@ -44,6 +45,9 @@ def _L():
         L.cldn_b200_viz_lossy_preprocess.argtypes = [vp, C.POINTER(_CInfo), vp, sz, vp, sz, C.POINTER(sz), C.POINTER(C.c_int), C.c_int]
         L.cldn_b200_viz_lossy_preprocess_batch.argtypes = [vp, C.POINTER(_CInfo), sz, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp),
                                                            C.POINTER(sz), C.POINTER(sz), C.POINTER(C.c_int), C.POINTER(_CInfo), C.c_int]
+        L.cldn_b200_preproc_prepare_batch.argtypes = [vp, C.POINTER(_CInfo), sz, C.c_uint64, C.POINTER(_CInfo)]
+        L.cldn_b200_viz_lossy_preprocess_batch_async.argtypes = [vp, sz, vp, vp, vp, vp, vp]
+        L.cldn_b200_preproc_sync.argtypes = [vp]
         L.cldn_b200_ros_parse.argtypes = [vp, sz, C.POINTER(_CRosMsg)]
         L.cldn_b200_ros_to_encoding_info.argtypes = [C.POINTER(_CRosMsg), C.POINTER(_CInfo)]
         L.cldn_b200_ros_apply_resolution_profile.argtypes = [C.POINTER(_CField), C.POINTER(C.c_uint32), C.POINTER(C.c_char_p),
@@ -286,6 +290,43 @@ class VizPreprocessor:
         """Device-pointer variant of run_batch: returns one (new_info, kept_points, applied) per cloud; survivors are at
         out_ptrs[f]."""
         return self._batch(info, len(in_ptrs), in_ptrs, in_bytes, out_ptrs, out_caps, MEM_DEVICE)
+
+    def prepare_batch(self, info: EncodingInfo, max_frames: int, max_points: int) -> EncodingInfo:
+        """Prepares run_batch_async() for calls of at most `max_frames` device clouds of layout `info` with at most
+        `max_points` points each. Returns the layout of an applied frame with width = height = 0 (``info`` itself for a
+        layout the preprocessing leaves alone): the EncodingInfo of the encoder that follows. See
+        cldn_b200_preproc_prepare_batch."""
+        c, after = _to_c(info), _CInfo()
+        _check(_L().cldn_b200_preproc_prepare_batch(self._h, C.byref(c), max_frames, max_points, C.byref(after)))
+        new_info = _from_c(after)
+        new_info.use_threads = info.use_threads
+        return new_info
+
+    def run_batch_async(self, frames_ptr: int, n: int, status_ptr: int, kept_ptr: int = 0, applied_ptr: int = 0,
+                        encode_descs_ptr: int = 0):
+        """Enqueues the preprocessing of n device clouds on the handle's stream and returns (graph capturable).
+        frames_ptr: device address of n descriptors (pack_viz_descs); status_ptr: device int32[n]; kept_ptr: device
+        uint64[n] or 0; applied_ptr: device int32[n] or 0; encode_descs_ptr: device address of n cloud descriptors
+        (cloudini_b200.pack_cloud_descs) whose cloud and size the call points at each frame's result, or 0. See
+        cldn_b200_viz_lossy_preprocess_batch_async."""
+        _check(_L().cldn_b200_viz_lossy_preprocess_batch_async(self._h, n, frames_ptr or None, status_ptr or None, kept_ptr or None,
+                                                               applied_ptr or None, encode_descs_ptr or None))
+
+    def sync(self):
+        """Waits for the handle's stream."""
+        _check(_L().cldn_b200_preproc_sync(self._h))
+
+
+def viz_descs(descs):
+    """numpy uint64 array [n, 4] of cldn_viz_desc_t: one (cloud_ptr, cloud_bytes, out_ptr, capacity) per frame, device
+    addresses and sizes as run_batch_async() reads them (the layout of cldn_blob_desc_t)."""
+    return blob_descs(descs)
+
+
+def pack_viz_descs(descs, out=None):
+    """The descriptors of viz_descs() in device memory, as pack_blob_descs() places them (32 bytes per frame). Returns
+    the tensor; its data_ptr() is run_batch_async()'s frames_ptr."""
+    return pack_blob_descs(descs, out)
 
 
 def applyVizLossyPreprocessing(pc: RosPointCloud2, preprocessor: Optional[VizPreprocessor] = None) -> None:

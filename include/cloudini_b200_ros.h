@@ -50,6 +50,61 @@ int cldn_b200_viz_lossy_preprocess_batch(cldn_preproc_t* pp, const cldn_info_t* 
                                          const size_t* out_capacities, size_t* kept_points, int* applied,
                                          cldn_info_t* infos_out, int mem);
 
+/* Device-resident clouds of ONE layout and any point counts, preprocessed without the host, so that the converter step
+ * (preprocessing, then cldn_b200_encode_blobs_async) runs on device pointers and can be captured in one CUDA graph.
+ *
+ * cldn_b200_preproc_prepare_batch: once per layout and shape, outside any capture. Width and height of `info` are
+ * ignored. It decides from the layout alone whether the reference's early returns apply (no xyz triple, or a resolution
+ * that is not positive and finite: a no-op layout). It allocates every device buffer a call of up to `max_frames`
+ * clouds of up to `max_points_per_frame` points needs, apart from the buffers of the handle's single and batch calls:
+ * a table region of 2 * max_points slots (rounded up to 1024) of 12 bytes, 4 bytes of slot per point and the tile
+ * status words, per frame: about 28 bytes per point of max_frames * max_points_per_frame (none for a no-op layout).
+ * `info_after` (optional) receives the layout an applied frame's infos_out[f] has, with width = height = 0 (every
+ * FLOAT64 field without a resolution gets 1e-6), or *info for a no-op layout: cldn_b200_encoder_create(info_after, ...)
+ * gives the encoder the chain needs. Refuses max_frames == 0 or >= 2^31 (CLDN_ERR_INVALID_ARGUMENT),
+ * max_points_per_frame > 2^30, the single call's limit, and shapes of 2^31 insert blocks or compaction tiles or more
+ * (CLDN_ERR_UNSUPPORTED). Waits for the handle's stream. A new prepare replaces the previous state; graphs captured
+ * before it are then invalid. cldn_b200_viz_lossy_preprocess and _batch keep working and do not disturb it.
+ *
+ * cldn_b200_viz_lossy_preprocess_batch_async: enqueues on the handle's stream and returns. No host synchronisation,
+ * allocation, pageable copy or host->device copy; the launches and their grids depend only on the prepared layout and
+ * shape, not on n_frames or on the point counts. Returns CLDN_ERR_INVALID_ARGUMENT, before anything is enqueued, without
+ * a prepared layout, with n_frames > max_frames, or with d_frames or d_status NULL; n_frames == 0 is CLDN_OK with no
+ * work. `d_frames`: DEVICE array of n_frames cldn_viz_desc_t. For every frame f < n_frames, d_status[f] (int32),
+ * d_kept[f] (uint64, optional) and d_applied[f] (int32, optional) are what cldn_b200_viz_lossy_preprocess(...,
+ * CLDN_MEM_DEVICE) returns and writes for that cloud alone, with its checks in its order:
+ *   CLDN_ERR_INVALID_ARGUMENT  a NULL cloud with cloud_bytes > 0; xyz fields outside the point (non-empty clouds);
+ *   CLDN_ERR_UNSUPPORTED       more than 2^30 points;
+ *   CLDN_ERR_BUFFER_TOO_SMALL  a NULL `out`, or capacity < points * point_step;
+ * and, checked last, the one refusal of this call alone:
+ *   CLDN_ERR_UNSUPPORTED       a non-empty cloud of an applying layout with more points than max_points_per_frame.
+ * A failed frame gets kept = cloud_bytes / point_step and applied = 0, as the single call leaves them. Survivors go to
+ * out[0, kept * point_step); no other byte of `out` is written, and a no-op or failed frame's output is untouched.
+ * Nothing of the frames >= n_frames is read or written.
+ * `d_encode` (optional): DEVICE array of n_frames cldn_cloud_desc_t whose out / capacity the caller set, for the blobs.
+ * The call writes only cloud, cloud_bytes, width and height of each:
+ *   applied:         cloud = out,   cloud_bytes = kept * point_step, width = height = 0;
+ *   OK, not applied: cloud = cloud, cloud_bytes = cloud_bytes,       width = height = 0;
+ *   failed:          cloud = NULL,  cloud_bytes = 1,                 width = height = 0, which
+ *                    cldn_b200_encode_blobs_async refuses with CLDN_ERR_INVALID_ARGUMENT before writing anything.
+ * cldn_b200_encode_blobs_async(enc, n_frames, d_encode, ...) enqueued behind it on the same stream, with `enc` created
+ * from info_after, then gives every good frame the blob cldn_b200_viz_lossy_preprocess_batch + cldn_b200_encode_blobs
+ * (widths = heights = NULL) give it.
+ *
+ * cldn_b200_preproc_sync: waits for the handle's stream and reports its CUDA error. */
+typedef struct cldn_viz_desc_t { /* all device pointers */
+  const void* cloud;
+  uint64_t cloud_bytes;
+  void* out;                      /* survivors; must not overlap `cloud` */
+  uint64_t capacity;
+} cldn_viz_desc_t;
+int cldn_b200_preproc_prepare_batch(cldn_preproc_t* pp, const cldn_info_t* info, size_t max_frames,
+                                    uint64_t max_points_per_frame, cldn_info_t* info_after);
+int cldn_b200_viz_lossy_preprocess_batch_async(cldn_preproc_t* pp, size_t n_frames, const void* d_frames,
+                                               int32_t* d_status, uint64_t* d_kept, int32_t* d_applied,
+                                               cldn_cloud_desc_t* d_encode);
+int cldn_b200_preproc_sync(cldn_preproc_t* pp);
+
 /* ---- N2: DDS envelope ------------------------------------------------------------------------------------------- */
 /* Parsed view of a CDR-serialised sensor_msgs/msg/PointCloud2 or point_cloud_interfaces/msg/CompressedPointCloud2
  * (cloudini_ros::RosPointCloud2, ros_msg_utils.hpp:32-148). `frame_id` and `data` are views (into the message that was
